@@ -1,7 +1,13 @@
-"""bench.py — NSF log_prob throughput on B200 (BASELINE.json metric).
+"""bench.py — NSF log_prob throughput on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA engine)
     python bench.py --impl reference --gpus N --steps K ...  # CPU arm (oracle port, host cores)
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's log_prob
+
+With --dump-outputs DIR, rank 0 writes what its last timed step returned: DIR/log_prob.npy (float32,
+one per row; above 64 MB a fixed seeded sample of rows, indices in log_prob_rows.npy) and
+DIR/sum_log_prob.npy (float64).  Weights and inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 
 A "step" is one pass of the hot path over one batch of synthetic input:
 ``flow(c).log_prob(x)`` + the fixed-order sum of the log-densities (the per-device term of
@@ -60,7 +66,8 @@ def measured_peaks() -> dict:
         d = json.loads(f.read_text())
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}  # fmt: skip
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 — upper bounds, not measurements
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "datasheet"}
 
 
 class ClockSampler:
@@ -314,9 +321,9 @@ def build_config_model(cfg):
 def tensor_peak(peaks: dict, clocks: dict) -> tuple[float, str]:
     """The denominator of a tensor-bound roofline: the measured cuBLAS burst figure (taken at the maximum SM clock) when
     the run held >= 98 % of that clock, else the same figure scaled to the clock the run actually held — the pipe's
-    capacity under the power cap the timed region saw.  (MEASURED_PEAKS.json's own "sustained" figure was taken at one
-    particular capped clock, 1305 MHz in round 1: dividing a run at 1935 MHz by it flatters, a run at 1680 MHz reads
-    above 1.  It is reported next to the fraction as `peak_sustained`.)"""
+    capacity under the power cap the timed region saw.  (A "sustained" figure in MEASURED_PEAKS.json is taken at one
+    particular capped clock: dividing a run at a higher clock by it flatters, a run at a lower clock can read above 1.
+    It is reported next to the fraction as `peak_sustained`.)"""
     sm, smax = clocks.get("sm_mhz"), clocks.get("sm_max_mhz")
     burst = peaks["bf16_tflops"]
     if not sm or not smax or sm >= 0.98 * smax:
@@ -335,7 +342,7 @@ def fused_info(flow) -> dict:
     for layer in flow.transform.transforms:
         out = (ctypes.c_double * 4)()
         k = E.lib().zk_layer_fused_info(layer._zk_layer(), out)
-        kinds.append({0: "per-layer GEMM kernels", 1: "fused_layer_kernel", 2: "fused_wide_kernel", 3: "fused_dual_kernel"}.get(k, "?"))
+        kinds.append({0: "per-layer GEMM kernels", 1: "fused_layer_kernel"}.get(k, "?"))
         issued += out[2]
         dense += out[3]
         entries += int(out[1])
@@ -345,7 +352,7 @@ def fused_info(flow) -> dict:
 def time_config(cfg, dev, rank, world, peaks, steps, nvml=None) -> dict:
     """One BASELINE configuration: warm-up, `steps` timed steps (CUDA events, max over ranks), oracle
     parity on a small slice (rank 0), roofline entry.  Inputs live in HBM; they rotate over buffers
-    that together exceed the 126 MB L2."""
+    that together exceed the 50 MB L2."""
     import torch.distributed as dist
 
     from zuko_b200 import _engine as E
@@ -355,7 +362,7 @@ def time_config(cfg, dev, rank, world, peaks, steps, nvml=None) -> dict:
     flow_cpu = build_config_model(cfg)
     flow = build_config_model(cfg).to(dev)
     g = torch.Generator(device=dev).manual_seed(4321 + rank)
-    nbuf = max(1, min(4, -(-(160 << 20) // (rows * (D + C) * 4))))  # > 126 MB in rotation
+    nbuf = max(1, min(4, -(-(160 << 20) // (rows * (D + C) * 4))))  # > 50 MB L2 in rotation
     xs = [torch.randn(rows, D, generator=g, device=dev) for _ in range(nbuf)]
     cs = [torch.randn(rows, C, generator=g, device=dev) for _ in range(nbuf)] if C else [None] * nbuf
     ring = NllRing(dev, slots=32)
@@ -427,13 +434,14 @@ def time_config(cfg, dev, rank, world, peaks, steps, nvml=None) -> dict:
             out["roofline"]["traffic_captured_at"] = ncu_traffic().get("git_sha")
     else:
         # every weight of the masked conditioner is visited once per sample (ar_inverse.cu): 2 FLOP per
-        # non-zero weight; roofline = fp32 FMA pipe, 148 SMs x 128 lanes x 2 x SM clock (nominal)
+        # non-zero weight; roofline = fp32 FMA pipe, SMs x 128 lanes x 2 x SM clock (nominal)
         nnz = sum(float(m.mask.sum()) for layer in flow_cpu.transform.transforms for m in layer.hyper if hasattr(m, "mask"))
         flops = 2.0 * nnz * rows
-        smax = clocks.get("sm_max_mhz") or 1965.0
-        peak = 148 * 128 * 2 * smax * 1e6 / 1e12
+        smax = clocks.get("sm_max_mhz") or torch.cuda.get_device_properties(dev).clock_rate / 1e3
+        sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        peak = sms * 128 * 2 * smax * 1e6 / 1e12
         tf = flops / (ms_per_step * 1e-3) / 1e12
-        out["roofline"] = {"bound": "fma", "achieved": tf, "peak": peak, "unit": "TFLOP/s", "frac": tf / peak, "peak_kind": "nominal fp32 FMA (148 SMs x 128 lanes x 2 x max SM clock)",
+        out["roofline"] = {"bound": "fma", "achieved": tf, "peak": peak, "unit": "TFLOP/s", "frac": tf / peak, "peak_kind": f"nominal fp32 FMA ({sms} SMs x 128 lanes x 2 x max SM clock)",
                            "kernel": ["ar_inverse_kernel<RQS,16>"], "algorithmic_flops_per_step": flops, "traffic": None,
                            "algorithmic_hbm_bytes": 4.0 * 2 * D * rows}  # fmt: skip
         tj = ncu_traffic().get(f"{cfg['name']}_layer")
@@ -472,7 +480,7 @@ def run_ours(args) -> None:
     peaks = measured_peaks()
 
     flow = build_model().to(dev)
-    NBUF = 4  # inputs rotate over 4 buffers: 4 x 100 MB > 126 MB L2
+    NBUF = 4  # inputs rotate over 4 buffers: 4 x 100 MB > 50 MB L2
     g = torch.Generator().manual_seed(1234 + rank)
     xs_host = [torch.randn(B, D, generator=g).pin_memory() for _ in range(NBUF)]
     cs_host = [torch.randn(B, C, generator=g).pin_memory() for _ in range(NBUF)]
@@ -486,8 +494,7 @@ def run_ours(args) -> None:
 
     def step(i: int):
         d = flow(cs[i % NBUF])
-        lp, _ = d.log_prob_and_sum(xs[i % NBUF], sum_out=ring.slot(B))
-        return lp
+        return d.log_prob_and_sum(xs[i % NBUF], sum_out=ring.slot(B))  # (log p per row, sum log p in a ring slot)
 
     with torch.no_grad():
         # ---- parity of the bench workload against the oracle (small slice, outside timing)
@@ -518,7 +525,7 @@ def run_ours(args) -> None:
             torch.cuda.synchronize()
             e0.record()
             for i in range(args.steps):
-                step(i)
+                last = step(i)
             nll_means = ring.means()  # waits for the outstanding mean-NLL collectives: inside the timed region
             e1.record()
             torch.cuda.synchronize()
@@ -531,6 +538,8 @@ def run_ours(args) -> None:
         ms_per_step = elapsed_ms.item() / args.steps
         value = world * B / (ms_per_step * 1e-3)
         nll_value = float(nll_means[-1].item())
+        if args.dump_outputs and rank == 0:
+            dump_outputs(Path(args.dump_outputs), *last)
 
         # ---- end to end through the public API with HOST buffers (H2D + compute + D2H per step)
         fc = flow(cs[0])._flow_call()[0]
@@ -607,7 +616,7 @@ def run_ours(args) -> None:
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32 (conditioner GEMMs: %s)" % gemm_mode_name(flow), "data": "synthetic",
             "config": {"workload": WORKLOAD, "batch_per_gpu": B, "global_batch": B * world,
-                       "parallelism": f"dp{world}", "l2": f"inputs rotate over {NBUF} buffers ({NBUF * B * (D + C) * 4 >> 20} MB > 126 MB L2)"},
+                       "parallelism": f"dp{world}", "l2": f"inputs rotate over {NBUF} buffers ({NBUF * B * (D + C) * 4 >> 20} MB > 50 MB L2)"},
             "clocks": clk.summary(), "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": B * (D + C) * 4, "d2h_bytes_per_step": B * 4,
                                              "steps": e2e_steps, "api": "FlowCall.log_prob_host -> zk_flow_log_prob_host (pinned host buffers)"},
             "gpu_launches": int(launches), "mean_nll": nll_value, "roofline": roofline, "kernels": kernels,
@@ -616,6 +625,24 @@ def run_ours(args) -> None:
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: Path, lp: torch.Tensor, total: torch.Tensor) -> None:
+    """What the last timed step returned to its caller: log p per row (float32) and the fixed-order
+    sum of log p (float64).  A batch whose log p exceeds the 64 MB budget is written as a fixed,
+    seeded sample of rows, with the row indices beside it (log_prob_rows.npy, float64)."""
+    out_dir.mkdir(parents=True, exist_ok=True)
+    lp = lp.float().cpu().numpy()
+    if lp.nbytes > DUMP_MAX_BYTES - (1 << 20):
+        n = (DUMP_MAX_BYTES - (1 << 20)) // 12  # float32 value + float64 index per sampled row
+        rows = np.sort(np.random.default_rng(0).choice(lp.shape[0], size=n, replace=False))
+        lp = lp[rows]
+        np.save(out_dir / "log_prob_rows.npy", rows.astype(np.float64))
+    np.save(out_dir / "log_prob.npy", lp)
+    np.save(out_dir / "sum_log_prob.npy", np.asarray(total.double().cpu().numpy(), dtype=np.float64).reshape(1))
 
 
 def time_training_step(flow, x, c, rows: int, iters: int) -> dict:
@@ -647,7 +674,7 @@ def time_training_step(flow, x, c, rows: int, iters: int) -> dict:
     return {"workload": WORKLOAD.replace("log_prob", "training step (log_prob forward + backward + Adam step)"), "rows": rows,
             "ms_per_step": ms, "samples_per_s": rows / (ms * 1e-3), "gpu_launches_per_step": launches,
             "algorithmic_tflops": 4 * flops / (ms * 1e-3) / 1e12, "optimizer_step_in_timed_region": True,
-            "note": "forward + recompute + dgrad + wgrad = 4 x the dense conditioner FLOPs; backward GEMMs on linear_tc_kernel (tcgen05 split-bf16); "
+            "note": "forward + recompute + dgrad + wgrad = 4 x the dense conditioner FLOPs; backward GEMMs on linear_tc_kernel (wgmma split-bf16); "
                     "gpu_launches_per_step counts engine kernels only (Adam's own kernels are torch's)"}  # fmt: skip
 
 
@@ -655,7 +682,7 @@ def gemm_mode_name(flow) -> str:
     from zuko_b200 import _engine as E
 
     h = flow.transform.transforms[0].hyper._handle()
-    return {E.ZK_GEMM_FP32: "fp32 FMA", E.ZK_GEMM_BF16X3: "tcgen05 bf16x3, fp32 accumulate", E.ZK_GEMM_BF16X1: "tcgen05 bf16"}.get(E.lib().zk_mlp_gemm_mode(h), "?")
+    return {E.ZK_GEMM_FP32: "fp32 FMA", E.ZK_GEMM_BF16X3: "wgmma bf16x3, fp32 accumulate", E.ZK_GEMM_BF16X1: "wgmma bf16"}.get(E.lib().zk_mlp_gemm_mode(h), "?")
 
 
 def ncu_traffic() -> dict:
@@ -701,8 +728,7 @@ def time_kernels(flow, x, c, dev, peaks, iters: int, peak_tf: float | None = Non
     peak_tf = peak_tf or peaks["bf16_tflops_sustained"]
     info = fused_info(flow)
     issued = 2.0 * info["issued_macs_per_row"] / T * B  # one flow layer, from the pack's tile table
-    fused_name = {"fused_wide_kernel": "fused_wide_kernel<RQS,8> (CTA pairs, cta_group::2)",
-                  "fused_dual_kernel": "fused_dual_kernel<RQS,8> (CTA pairs, two sub-tiles in flight)"}.get(info["kernel"][0], "fused_layer_kernel<RQS,8>")
+    fused_name = "fused_layer_kernel<RQS,8>"
     n0 = L.zk_launch_count()
     fused()
     is_fused = (L.zk_launch_count() - n0) == 1
@@ -710,7 +736,7 @@ def time_kernels(flow, x, c, dev, peaks, iters: int, peak_tf: float | None = Non
         fused()
         t = cuda_time_ms(fused, iters)
         tf = flops / (t * 1e-3) / 1e12
-        out.append({"name": fused_name + " (conditioner 24-256-256-256-368 on tcgen05 + RQS + ladj), one flow layer",
+        out.append({"name": fused_name + " (conditioner 24-256-256-256-368 on wgmma + RQS + ladj), one flow layer",
                     "bound": "tensor", "achieved": tf, "peak": peak_tf, "peak_kind": peak_kind, "unit": "TFLOP/s",
                     "frac": tf / peak_tf, "traffic": traffic.get(info["kernel"][0] + "_cfg2", traffic.get("fused_layer_kernel") if info["kernel"][0] == "fused_layer_kernel" else None), "traffic_captured_at": traffic.get("git_sha"),
                     "ms_per_launch": t, "ms_per_step": t * T,
@@ -768,11 +794,15 @@ def main() -> None:
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--batch", type=int, default=1 << 20, help="rows per GPU")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step under DIR (rank 0; see the module docstring)")
     ap.add_argument("--cpu-rows", type=int, default=0, help="rows of the bounded CPU sample (0 = 2^19)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-training-step", action="store_true", help="skip the forward+backward timing (extra object)")
     ap.add_argument("--no-configs", action="store_true", help="skip the cfg3 / cfg4 / cfg5 entries of the line")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * zuko_b200 — C ABI of the B200-native (sm_100a) engine for Zuko's flow hot path.
+ * zuko_b200 — C ABI of the H100-native (sm_90a) engine for Zuko's flow hot path.
  *
  * The reference (probabilists/zuko @ 1063ae4) has NO FFI, plugin registry or
  * native code: its seams are Python protocols.  The entry points below are the
@@ -62,9 +62,9 @@ typedef void* zk_stream; /* cudaStream_t */
 #define ZK_LAYER_ROTATION 6       /* transforms.py:1217-1244 */
 
 /* arithmetic of the conditioner GEMMs (zuko/nn.py:217-218) */
-#define ZK_GEMM_AUTO 0    /* tcgen05 split-bf16 when the shape allows it, else fp32 SIMT */
+#define ZK_GEMM_AUTO 0    /* tensor-core split-bf16 when the shape allows it, else fp32 SIMT */
 #define ZK_GEMM_FP32 1    /* fp32 FMA on CUDA cores (exact-order reference path, any shape) */
-#define ZK_GEMM_BF16X3 2  /* tcgen05.mma kind::f16, bf16 hi/lo split (3 MMAs), fp32 accumulate in TMEM */
+#define ZK_GEMM_BF16X3 2  /* wgmma bf16, hi/lo split (3 MMAs), fp32 accumulate in registers */
 #define ZK_GEMM_BF16X1 3  /* single bf16 MMA: fast, does NOT meet the 1e-5 parity bar */
 
 /* activation between the linear layers of a conditioner (zuko/nn.py:264-265: `activation()` modules);
@@ -212,10 +212,9 @@ zk_status zk_layer_update_weights(zk_layer* layer, const float* const* weight, c
 void zk_set_pack_stream(zk_stream stream);
 size_t zk_layer_workspace_bytes(const zk_layer* layer, int64_t B);
 /* Bench bookkeeping: which kernel runs an autoregressive layer's forward (flows/autoregressive.py:
- * 207-215) and how much tensor-core work its issue schedule holds.  Returns 0 = per-layer GEMM
- * kernels, 1 = fused layer kernel, 2 = wide fused layer kernel (CTA pairs), 3 = dual-tile CTA-pair
- * kernel; out[0] = the same,
- * out[1] = schedule entries per tile, out[2] = MACs ISSUED per sample row (non-zero tiles only, all
+ * 207-215) and how much tensor-core work it issues.  Returns 0 = per-layer GEMM kernels,
+ * 1 = fused layer kernel; out[0] = the same,
+ * out[1] = non-zero 64 x 64 weight tiles per row tile, out[2] = MACs ISSUED per sample row (non-zero tiles only, all
  * split-bf16 terms), out[3] = dense MACs per sample row (what nn.py:218 executes). */
 int zk_layer_fused_info(const zk_layer* layer, double* out);
 /* 1 when the layer's inverse runs as the dimension-sequential kernel (one launch, emits the ladj): the
@@ -392,7 +391,7 @@ zk_status zk_allreduce_sum(zk_comm* comm, int dev, double* buf, int n, zk_stream
 zk_status zk_comm_group_end(zk_comm* comm);
 
 /* 1 (default): the conditioner GEMMs of the backward pass (forward recompute, dgrad, wgrad) of a
- * handle packed for tcgen05 run on the tensor cores (split-bf16, fp32 accumulate); 0: fp32 FMA on
+ * handle packed for the tensor cores run on them (split-bf16, fp32 accumulate); 0: fp32 FMA on
  * CUDA cores (exact-order arbitration path).  Returns the previous value. */
 int zk_set_tc_backward(int on);
 
@@ -400,48 +399,14 @@ int zk_set_tc_backward(int on);
  * approximations, 0 = IEEE division + expf / logf.  Process-wide; returns the previous
  * value.  Both settings meet the 1e-5 parity bar on the BASELINE configs (tests/). */
 int zk_set_fast_math(int on);
-/* 1 (default): an autoregressive layer whose conditioner fits a fused kernel (hidden widths
- * equal; multiple of 64 and <= 256 with D + C <= 256, or 384 / 512 with D + C <= 512; RQS with
+/* 1 (default): an autoregressive layer whose conditioner fits the fused kernel (hidden widths
+ * equal, a multiple of 64 and <= 512; D + C <= 512; RQS with
  * 8 / 16 bins or affine; tensor-core GEMM mode; any supported activation, no residual blocks) runs as ONE kernel —
  * conditioner + bijector + ladj, activations and phi stay on chip (nn.py:217-218,
  * flows/autoregressive.py:207-215, transforms.py:554-567 in one launch).
  * 0: always one GEMM kernel per linear layer + the stand-alone bijector kernel.  Returns the
  * previous value. */
 int zk_set_fused_layers(int on);
-/* Smallest (equal) hidden width that is routed to the CTA-pair fused kernel (cta_group::2 MMAs, the only
- * one for widths 384 / 512): 256 (default) or 384 — with 384, width-256 conditioners run on the
- * one-CTA-per-tile kernel as in round 1.  Applies to handles created afterwards.  Returns the previous value. */
-int zk_set_wide_min_hidden(int h);
-/* 1 (default): conditioners of (equal) hidden width 128 / 256 with D + C <= 256 run on the dual-tile
- * CTA-pair kernel (two 128-row sub-tiles in flight per CTA: the MMAs of one overlap the epilogue of the
- * other); 0: the one-tile kernels as before.  Applies to handles created afterwards.  Returns the previous value. */
-int zk_set_dual_tiles(int on);
-/* Profiling hook: a DEVICE buffer of >= 256 int64 that the fused layer kernel fills with clock64()
- * stamps of its pipeline events (CTA 0, third tile); NULL (default) disables it. */
-void zk_debug_timeline(long long* device_buffer);
-
-/* Host-only (no CUDA call): the issue schedule the wide fused kernel (hidden width 384 / 512) would
- * walk for a conditioner with layer widths dims[0..n_linear] and HOST masks (bool bytes
- * (dims[l+1], dims[l]) row-major, NULL = dense) — nn.py:270-293 builds those masks.  Writes two
- * words per entry (flags, first weight row; bit layout in csrc/fused_wide.cu), the K blocks each
- * layer reads (out_rd_mask[8], may be NULL) and the degree-sort permutations of the hidden layers
- * concatenated (out_perm, may be NULL).  Returns the number of entries; -1 shape not supported,
- * -2 the protocol dry run rejected the schedule, -3 max_items too small. */
-int zk_debug_wide_schedule(int n_linear, const int* dims, const uint8_t* const* masks_host, int univariate, int bins,
-                           int features, int context, uint32_t* out_items, int max_items, uint32_t* out_rd_mask,
-                           int* out_perm);
-/* Same for the dual-tile kernel (hidden width 128 / 256): the schedule of one 512-row pair tile, entries of
- * the two sub-tiles interleaved chunk by chunk (bit 2 of the flags = sub-tile; csrc/fused_dual.cu). */
-int zk_debug_dual_schedule(int n_linear, const int* dims, const uint8_t* const* masks_host, int univariate, int bins,
-                           int features, int context, uint32_t* out_items, int max_items, uint32_t* out_rd_mask,
-                           int* out_perm);
-/* Debugging aid of the wide fused kernel: every wait inside it is bounded (~2 s); a wait that
- * expires reports its role, barrier and position in the schedule into pinned host memory and
- * traps.  Copies up to n_words 32-bit words of that report into `out` (word 0 = number of
- * reports, 8 words per (CTA of cluster 0, warp) from word 8); returns the number of words
- * copied, 0 when no wide kernel was launched yet.  Readable after the context died. */
-int zk_debug_watchdog_read(uint32_t* out, int n_words);
-
 /* number of kernel launches issued by this library since load (bench evidence) */
 int64_t zk_launch_count(void);
 

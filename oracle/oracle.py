@@ -41,7 +41,7 @@ def build(force: bool = False) -> Path:
         return _LIB_PATH
     cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
     base = [cc, "-O3", "-fPIC", "-shared", str(src), "-o", str(_LIB_PATH), "-lm"]
-    # AVX2 + FMA (every x86 host of a B200 has them) and OpenMP when the toolchain allows;
+    # AVX2 + FMA (every x86 host of an H100 has them) and OpenMP when the toolchain allows;
     # no -ffast-math: the fp32 variant must round like the reference's eager ops.
     for extra in (["-mavx2", "-mfma", "-fopenmp"], ["-fopenmp"], []):
         try:

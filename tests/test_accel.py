@@ -1,18 +1,18 @@
 """`zuko_b200.accelerate(flow)` — the drop-in seam of SURVEY §8(b): an engine-backed
 LazyDistribution that shares the parameters / buffers of an existing flow.
 
-CPU part: structure, sharing and error behaviour, against flows built by the *unmodified
-reference* when it is importable in this container (it is not on the GPU box) and against the
-engine's own modules otherwise.  GPU part: the accelerated flow reproduces the golden
-log-densities and follows in-place updates of the source flow.
+CPU part: structure, sharing and error behaviour.  The flows of `_flows` are built with the engine's
+constructors under the seed the reference used for tests/golden/accel_reference.npz
+(make_golden_accel.py), so the accelerated flows are held to the reference's own state dicts, orders and
+masks.  GPU part: the accelerated flow reproduces the golden log-densities and follows in-place updates
+of the source flow.
 """
 
 from __future__ import annotations
 
-import os
-import sys
 from functools import partial
 
+import numpy as np
 import pytest
 import torch
 
@@ -21,21 +21,9 @@ from zuko_b200.accel import _convert, _share
 
 from cases import SMALL_CASES, assert_log_prob_parity, build_flow, load
 
-REFERENCE = "/root/reference"
 
-
-def _reference():
-    if not os.path.isdir(os.path.join(REFERENCE, "zuko")):
-        pytest.skip("reference sources are not present on this machine")
-    sys.dont_write_bytecode = True
-    if REFERENCE not in sys.path:
-        sys.path.append(REFERENCE)
-    import zuko
-
-    return zuko
-
-
-def _reference_flows(zuko):
+def _flows(zuko):
+    """The same flows from either package (the reference's `zuko` or `zuko_b200`), seeded."""
     torch.manual_seed(0)
     F, T, D = zuko.flows, zuko.transforms, zuko.distributions
     base = lambda n: F.UnconditionalDistribution(D.DiagNormal, torch.zeros(n), torch.ones(n), buffer=True)  # noqa: E731
@@ -64,6 +52,20 @@ def _reference_flows(zuko):
     }  # fmt: skip
 
 
+@pytest.fixture(scope="module")
+def golden():
+    return load("accel_reference")
+
+
+def _assert_reference_state(flow, golden, name):
+    """`flow`'s state dict is the one the reference built: same keys in the same order, same tensors."""
+    sd = flow.state_dict()
+    assert list(sd) == [str(k) for k in golden[f"{name}/keys"]], name
+    for i, (k, t) in enumerate(sd.items()):
+        ref = golden[f"{name}/sd/{i:03d}"]
+        assert tuple(t.shape) == ref.shape and np.array_equal(t.detach().cpu().numpy(), ref), (name, k)
+
+
 def _assert_shared(acc, src):
     sd_src, sd_acc = src.state_dict(), acc.state_dict()
     assert list(sd_src) == list(sd_acc)
@@ -75,38 +77,41 @@ def _assert_shared(acc, src):
     assert all(b_src[k] is b_acc[k] for k in b_src)
 
 
-def test_accelerate_reference_flows_share_tensors():
-    zuko = _reference()
-    for name, src in _reference_flows(zuko).items():
+def test_accelerate_reference_flows_share_tensors(golden):
+    for name, src in _flows(zuko_b200).items():
+        _assert_reference_state(src, golden, name)
         acc = zuko_b200.accelerate(src)
         assert isinstance(acc, zuko_b200.lazy.LazyDistribution), name
         _assert_shared(acc, src)
-        # every lazy layer was replaced by its engine counterpart
+        _assert_reference_state(acc, golden, name)
+        # every lazy layer is an engine module
         for t in acc.transform.transforms:
             assert type(t).__module__.startswith("zuko_b200."), (name, type(t))
 
 
-def test_accelerate_keeps_reference_built_masks_and_orders():
-    zuko = _reference()
-    src = _reference_flows(zuko)["maf_randperm"]
+def test_accelerate_keeps_reference_built_masks_and_orders(golden):
+    flows = _flows(zuko_b200)
+    src = flows["maf_randperm"]
     acc = zuko_b200.accelerate(src)
-    for ts, ta in zip(src.transform.transforms, acc.transform.transforms, strict=True):
-        assert ta.passes == ts.passes and torch.equal(ta.order, ts.order)
-        for ms, ma in zip(ts.hyper, ta.hyper, strict=True):
+    for i, (ts, ta) in enumerate(zip(src.transform.transforms, acc.transform.transforms, strict=True)):
+        assert ta.passes == ts.passes == int(golden[f"maf_randperm/passes/{i}"])
+        assert torch.equal(ta.order, ts.order) and np.array_equal(ta.order.numpy(), golden[f"maf_randperm/order/{i}"])
+        for j, (ms, ma) in enumerate(zip(ts.hyper, ta.hyper, strict=True)):
             if hasattr(ms, "mask"):
                 assert ma.mask is ms.mask
-    adj = zuko_b200.accelerate(_reference_flows(zuko)["adjacency"])
-    assert adj.transform.transforms[0].order is None and adj.transform.transforms[0].passes == 3
+                assert np.array_equal(ma.mask.numpy(), golden[f"maf_randperm/mask/{i}/{j}"])
+    adj = zuko_b200.accelerate(flows["adjacency"])
+    assert adj.transform.transforms[0].order is None
+    assert adj.transform.transforms[0].passes == int(golden["adjacency/passes/0"]) == 3
 
 
 def test_accelerate_sees_updates_of_the_source():
-    zuko = _reference()
-    src = _reference_flows(zuko)["nsf"]
+    src = _flows(zuko_b200)["nsf"]
     acc = zuko_b200.accelerate(src)
     layer = acc.transform.transforms[0]
     sig0 = layer._layer_signature()
     with torch.no_grad():
-        src.transform.transforms[0].hyper[0].weight.mul_(1.5)  # an optimizer step on the reference module
+        src.transform.transforms[0].hyper[0].weight.mul_(1.5)  # an optimizer step on the source module
     assert layer._layer_signature() != sig0  # -> the packed weights are rebuilt on the next call
     # load_state_dict on the source copies in place: still shared
     src.load_state_dict({k: torch.zeros_like(v) for k, v in src.state_dict().items()})
@@ -118,10 +123,20 @@ def test_accelerate_sees_updates_of_the_source():
     _assert_shared(acc, src)
 
 
+class NeuralAutoregressiveTransform(zuko_b200.lazy.LazyTransform):
+    """Stand-in with the name of a reference transform the engine does not implement (NAF's layer)."""
+
+    def forward(self, c=None):  # noqa: ANN001, ANN201
+        raise AssertionError("never called")
+
+
 def test_accelerate_rejects_what_the_engine_does_not_implement():
-    zuko = _reference()
-    F = zuko.flows
-    for bad in (F.MAF(3, 0, activation=torch.nn.PReLU), F.NAF(3, 0), F.GF(3, 0)):
+    F = zuko_b200.flows
+    prelu = F.MAF(3, 0)
+    for t in prelu.transform.transforms:  # a conditioner activation the engine has no kernel for
+        t.hyper[1] = torch.nn.PReLU()
+    base = F.UnconditionalDistribution(zuko_b200.distributions.DiagNormal, torch.zeros(3), torch.ones(3), buffer=True)
+    for bad in (prelu, F.Flow([NeuralAutoregressiveTransform()], base)):
         with pytest.raises(NotImplementedError, match="accelerate"):
             zuko_b200.accelerate(bad)
     with pytest.raises(TypeError, match="float32"):

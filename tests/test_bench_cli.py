@@ -57,9 +57,9 @@ def test_tensor_roofline_denominator_follows_the_clock():
     sys.path.insert(0, str(ROOT))
     import bench
 
-    peaks = {"bf16_tflops": 1640.0, "bf16_tflops_sustained": 1368.6}
-    assert bench.tensor_peak(peaks, {"sm_mhz": 1965.0, "sm_max_mhz": 1965.0, "reasons": []}) == (1640.0, "burst")
-    assert bench.tensor_peak(peaks, {"sm_mhz": 1935.0, "sm_max_mhz": 1965.0, "reasons": ["sw_power_cap"]}) == (1640.0, "burst")
-    peak, kind = bench.tensor_peak(peaks, {"sm_mhz": 1680.0, "sm_max_mhz": 1965.0, "reasons": ["sw_power_cap"]})
-    assert abs(peak - 1640.0 * 1680.0 / 1965.0) < 1e-9 and "1680" in kind and "burst" in kind
-    assert bench.tensor_peak(peaks, {}) == (1640.0, "burst")  # no NVML: nothing to scale by
+    peaks = {"bf16_tflops": 989.0, "bf16_tflops_sustained": 900.0}
+    assert bench.tensor_peak(peaks, {"sm_mhz": 1980.0, "sm_max_mhz": 1980.0, "reasons": []}) == (989.0, "burst")
+    assert bench.tensor_peak(peaks, {"sm_mhz": 1950.0, "sm_max_mhz": 1980.0, "reasons": ["sw_power_cap"]}) == (989.0, "burst")
+    peak, kind = bench.tensor_peak(peaks, {"sm_mhz": 1680.0, "sm_max_mhz": 1980.0, "reasons": ["sw_power_cap"]})
+    assert abs(peak - 989.0 * 1680.0 / 1980.0) < 1e-9 and "1680" in kind and "burst" in kind
+    assert bench.tensor_peak(peaks, {}) == (989.0, "burst")  # no NVML: nothing to scale by

@@ -5,7 +5,7 @@ against gradients that torch.autograd produced on the UNMODIFIED reference in fp
 
 Rows on which the flow is not differentiable to working precision (a hidden pre-activation within
 the GEMM's rounding error of the ReLU kink in the fp64 oracle, cases.relu_kink_rows — there a sign
-flip of the last bits changes the gradient by a finite jump; the tcgen05 split-bf16 conditioner and
+flip of the last bits changes the gradient by a finite jump; the tensor-core split-bf16 conditioner and
 the fp32 one each flip a handful of such units, as does the reference's own fp32 path) get zero weight, and the golden sums are corrected by
 the pinned gradient oracle for exactly those rows (gradients are linear in the per-row weights).
 
@@ -301,7 +301,7 @@ def test_chunked_backward_and_determinism(device):
 
 @pytest.mark.parametrize("name,B", [("cfg2_nsf", 6000), ("cfg5_nsf", 2500), ("cfg3_maf", 3000), ("cfg4_nsf", 1500)])
 def test_tensor_core_and_fp32_backward_agree(device, name, B):
-    """The tcgen05 split-bf16 backward (forward recompute, dgrad, batch-sliced wgrad) against the
+    """The tensor-core split-bf16 backward (forward recompute, dgrad, batch-sliced wgrad) against the
     fp32 CUDA-core backward of the same handle on a batch large enough for several batch slices,
     and both against the gradient oracle on the leading rows."""
     flow = build_flow(name).to(device)

@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 (tensor-core) conditioner path against the fp64 oracle and the
+"""GPU tests of the tensor-core (wgmma) conditioner path against the fp64 oracle and the
 fp32 CUDA-core path."""
 
 import ctypes
@@ -71,7 +71,7 @@ def test_bf16x1_is_available_but_inexact(device):
 
 @pytest.mark.parametrize("name", ["cfg2_nsf", "cfg3_maf", "cfg4_nsf", "cfg5_nsf", "nsf35_row", "nice35"])
 def test_flow_parity_on_tensor_cores(device, name):
-    """The BASELINE configs with the conditioner forced onto tcgen05 (bf16x3): log_prob within
+    """The BASELINE configs with the conditioner forced onto the tensor cores (bf16x3): log_prob within
     1e-5 relative of the reference."""
     g = load(f"flow_{name}")
     flow = build_flow(name, g)
@@ -94,7 +94,7 @@ RES_SHAPES = [
 @pytest.mark.parametrize("shape,hidden,act", RES_SHAPES)
 @pytest.mark.parametrize("B", [1, 129, 5000])
 def test_residual_mlp_on_tensor_cores(device, shape, hidden, act, B):
-    """MaskedMLP(residual=True) (zuko/nn.py:195-199, 297-309) on the tcgen05 GEMM kernels: the second layer of a
+    """MaskedMLP(residual=True) (zuko/nn.py:195-199, 297-309) on the tensor-core GEMM kernels: the second layer of a
     block adds the block's input, read back from the bf16 hi / lo planes the kernel overwrites in place."""
     def make():
         torch.manual_seed(5)
@@ -120,7 +120,7 @@ def test_residual_mlp_on_tensor_cores(device, shape, hidden, act, B):
 @pytest.mark.parametrize("name", ["res_nsf_relu", "res_nsf_mixed"])
 def test_residual_goldens_on_tensor_cores(device, name):
     """The reference's residual flows (tests/golden/make_golden_res.py) with the conditioner forced onto
-    tcgen05: log_prob within 1e-5 of the reference, gradients still flow (fp32 backward kernels)."""
+    the tensor cores: log_prob within 1e-5 of the reference, gradients still flow (fp32 backward kernels)."""
     g = load(f"flow_{name}")
     flow = build_flow(name, g)
     for t in flow.transform.transforms:
@@ -169,22 +169,22 @@ def test_auto_mode_picks_tensor_cores_for_wide_layers(device):
 FUSED_FLOWS = {
     "nsf16c8_h256": lambda: zuko.flows.NSF(16, 8, transforms=2, bins=8, hidden_features=[256] * 3),   # cfg2 shape
     "nsf64_k16_h64": lambda: zuko.flows.NSF(64, 0, transforms=2, bins=16),                             # cfg4 shape
-    "nsf5c3_h192": lambda: zuko.flows.NSF(5, 3, transforms=3, bins=8, hidden_features=[192, 192]),     # 64-wide chunks, D % 4 != 0
-    "nsf7_k16_h128": lambda: zuko.flows.NSF(7, 0, transforms=2, bins=16, hidden_features=[128, 128]),  # odd D with DPC = 2
-    "maf32_h256": lambda: zuko.flows.MAF(32, 0, transforms=2, hidden_features=[256] * 2),              # affine, 64 dims / chunk
-    "maf70c100_h128": lambda: zuko.flows.MAF(70, 100, transforms=2, hidden_features=[128] * 2),        # K0 = 170 -> 3 K blocks, 2 affine chunks
-    # ---- wide kernel (fused_wide.cu): hidden width 384 / 512 on CTA pairs, in-place descending schedule ----
+    "nsf5c3_h192": lambda: zuko.flows.NSF(5, 3, transforms=3, bins=8, hidden_features=[192, 192]),     # hidden width 192, odd D with DPC = 2
+    "nsf7_k16_h128": lambda: zuko.flows.NSF(7, 0, transforms=2, bins=16, hidden_features=[128, 128]),  # 16 bins: one dim per output chunk (DPC = 1)
+    "maf32_h256": lambda: zuko.flows.MAF(32, 0, transforms=2, hidden_features=[256] * 2),              # affine, 32 dims / chunk
+    "maf70c100_h128": lambda: zuko.flows.MAF(70, 100, transforms=2, hidden_features=[128] * 2),        # K0 = 170 -> 3 K blocks, 3 affine chunks
+    # ---- hidden width 384 / 512: four accumulators per warpgroup, activations overwritten in place ----
     "maf32_h512x4": lambda: zuko.flows.MAF(32, 0, transforms=2, hidden_features=[512] * 4),            # cfg3 shape
     "nsf64c16_k16_h512": lambda: zuko.flows.NSF(64, 16, transforms=2, bins=16, hidden_features=[512] * 3),  # cfg5 shape
     "nsf24_k8_h512": lambda: zuko.flows.NSF(24, 0, transforms=2, bins=8, hidden_features=[512, 512]),  # degree classes not aligned to chunks
     "nsf10c3_h384": lambda: zuko.flows.NSF(10, 3, transforms=3, bins=8, hidden_features=[384, 384]),   # 3 chunks / 6 K blocks
     "maf100c28_h512": lambda: zuko.flows.MAF(100, 28, transforms=2, hidden_features=[512] * 2),        # K0 = 128, 2 affine chunks
-    # ---- non-ReLU activations on the fused pair kernels (nn.py:264-265; general-activation instantiation) ----
+    # ---- non-ReLU activations (nn.py:264-265; general-activation instantiation) ----
     "maf32_h512_elu": lambda: zuko.flows.MAF(32, 0, transforms=2, hidden_features=[512] * 2, activation=torch.nn.ELU),
     "nsf16c8_h256_silu": lambda: zuko.flows.NSF(16, 8, transforms=2, bins=8, hidden_features=[256] * 2, activation=torch.nn.SiLU),
     "nsf12_h256_tanh": lambda: zuko.flows.NSF(12, 0, transforms=2, bins=8, hidden_features=[256, 256], activation=torch.nn.Tanh),
     "maf24c4_h384_gelu": lambda: zuko.flows.MAF(24, 4, transforms=2, hidden_features=[384] * 2, activation=torch.nn.GELU),
-    # ---- ... and on the one-CTA-per-tile kernel (hidden width 64 - 192, the library's default widths) ----
+    # ---- ... and at hidden width 64 - 192, the library's default widths ----
     "maf8_h64_tanh": lambda: zuko.flows.MAF(8, 0, transforms=2, activation=torch.nn.Tanh),
     "nsf5c3_h192_elu": lambda: zuko.flows.NSF(5, 3, transforms=2, bins=8, hidden_features=[192, 192], activation=torch.nn.ELU),
     "nsf20_k16_h64_silu": lambda: zuko.flows.NSF(20, 0, transforms=2, bins=16, activation=torch.nn.SiLU),
@@ -240,8 +240,7 @@ def test_fused_layer_matches_unfused_and_oracle(device, unfused, name, B):
 @pytest.mark.parametrize("name", ONE_LAUNCH_FLOWS)
 def test_wide_layers_run_as_one_kernel_each(device, name):
     """Hidden width 384 / 512, and non-ReLU conditioners of every fused width: ONE launch per flow layer (no
-    per-layer GEMM fallback), and a ragged
-    batch (partial pair tile, odd number of tiles) gives the rows of the full batch bit for bit."""
+    per-layer GEMM fallback), and a ragged batch (partial tile) gives the rows of the full batch bit for bit."""
     torch.manual_seed(5)
     flow = FUSED_FLOWS[name]().to(device)
     D = flow.base.loc.shape[0]
@@ -256,40 +255,6 @@ def test_wide_layers_run_as_one_kernel_each(device, name):
         assert E.lib().zk_launch_count() - n0 == len(flow.transform.transforms)
         lp_part = flow(None if c is None else c[:300]).log_prob(x[:300])
     assert torch.equal(lp[:300], lp_part)
-
-
-def test_the_three_fused_kernels_agree_on_cfg2(device):
-    """Hidden width 256 can run on all three fused kernels (one CTA per tile, CTA pair, CTA pair with two
-    sub-tiles in flight): same oracle parity, mutual agreement to rounding, one launch per layer each."""
-    torch.manual_seed(7)
-    ref_flow = zuko.flows.NSF(16, 8, transforms=2, bins=8, hidden_features=[256] * 3).eval()
-    spec = O.flowspec_from_module(ref_flow)
-    g = torch.Generator().manual_seed(3)
-    x, c = torch.randn(5000, 16, generator=g), torch.randn(5000, 8, generator=g)
-    ref = spec.log_prob(x.numpy(), c.numpy())
-    outs = {}
-    import ctypes
-
-    for name, dual, min_h, kind in (("narrow", 0, 384, 1), ("pair", 0, 256, 2), ("dual", 1, 256, 3)):
-        pd, pw = E.lib().zk_set_dual_tiles(dual), E.lib().zk_set_wide_min_hidden(min_h)
-        try:
-            flow = zuko.flows.NSF(16, 8, transforms=2, bins=8, hidden_features=[256] * 3)
-            flow.load_state_dict(ref_flow.state_dict())
-            flow = flow.to(device)
-            with torch.no_grad():
-                lp = flow(c.to(device)).log_prob(x.to(device))
-                n0 = E.lib().zk_launch_count()
-                lp = flow(c.to(device)).log_prob(x.to(device))
-                assert E.lib().zk_launch_count() - n0 == 2
-            info = (ctypes.c_double * 4)()
-            assert E.lib().zk_layer_fused_info(flow.transform.transforms[0]._zk_layer(), info) == kind
-        finally:
-            E.lib().zk_set_dual_tiles(pd)
-            E.lib().zk_set_wide_min_hidden(pw)
-        outs[name] = lp
-        assert rel_err(lp.cpu().numpy(), ref) < 1e-5, name
-    for name in ("pair", "dual"):
-        assert torch.allclose(outs[name], outs["narrow"], rtol=2e-6, atol=5e-5)
 
 
 def test_fused_layer_broadcast_context_and_launch_count(device):

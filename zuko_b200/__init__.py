@@ -1,4 +1,4 @@
-"""zuko_b200 — B200-native (sm_100a) log-density and sampling engine for Zuko's flow hot path.
+"""zuko_b200 — H100-native (sm_90a) log-density and sampling engine for Zuko's flow hot path.
 
 The public surface mirrors the reference (probabilists/zuko) for the hot path only:
 ``zuko_b200.flows.{MAF, NSF, NICE, ...}``, ``zuko_b200.lazy.Flow``,

@@ -105,13 +105,7 @@ _SIGNATURES = {
     "zk_launch_count": (c_int64, []),
     "zk_set_fast_math": (c_int, [c_int]),
     "zk_set_fused_layers": (c_int, [c_int]),
-    "zk_set_wide_min_hidden": (c_int, [c_int]),
-    "zk_set_dual_tiles": (c_int, [c_int]),
-    "zk_debug_dual_schedule": (c_int, [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "zk_set_tc_backward": (c_int, [c_int]),
-    "zk_debug_timeline": (None, [c_void_p]),
-    "zk_debug_watchdog_read": (c_int, [c_void_p, c_int]),
-    "zk_debug_wide_schedule": (c_int, [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "zk_device_info": (c_int, [POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "zk_rqs_forward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_float, c_float, _P, c_int64, _P, c_int, _P]),
     "zk_rqs_inverse": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_float, c_float, _P, c_int64, _P]),
@@ -180,7 +174,7 @@ def lib() -> ctypes.CDLL:
         if not LIB_PATH.exists():
             raise EngineError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). zuko_b200 has no CPU / eager fallback."
+                "(nvcc, sm_90a). zuko_b200 has no CPU / eager fallback."
             )
         handle = ctypes.CDLL(os.fspath(LIB_PATH))
         for name, (res, args) in _SIGNATURES.items():
@@ -210,8 +204,8 @@ def stream_ptr(device: torch.device) -> c_void_p:
 def require_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise EngineError(
-            f"zuko_b200: {what} lives on {t.device}; the engine only runs on CUDA (sm_100a) and has no "
-            "CPU fallback. Move the flow and its inputs to a B200 with .cuda()."
+            f"zuko_b200: {what} lives on {t.device}; the engine only runs on CUDA (sm_90a) and has no "
+            "CPU fallback. Move the flow and its inputs to an H100 with .cuda()."
         )
     if t.dtype != torch.float32:
         raise TypeError(f"zuko_b200: {what} has dtype {t.dtype}; the engine computes in float32 only")

@@ -1,4 +1,4 @@
-"""``accelerate(flow)`` — put the B200 engine behind an *existing* reference flow.
+"""``accelerate(flow)`` — put the H100 engine behind an *existing* reference flow.
 
 The reference has no plugin registry; its stable seam for the hot path is
 ``LazyDistribution.forward(c) -> Distribution`` (zuko/lazy.py:39-49, SURVEY §8b).

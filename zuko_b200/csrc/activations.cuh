@@ -30,7 +30,7 @@ ZK_ACT_HD float act_apply(float v, int act) {
 }
 
 // the same over N values with ONE switch outside the loops (inside an unrolled epilogue a per-element
-// switch multiplies the code size: mlp_tcgen05.cu learned that the hard way, DESIGN.md §5)
+// switch multiplies the code size and slows the epilogue through the instruction cache)
 template <int N>
 ZK_ACT_HD void act_apply_n(float (&v)[N], int act) {
     switch (act) {

@@ -32,10 +32,10 @@ zk_status fail(zk_status code, const char* fmt, ...) {
 int sm_count() {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (cached[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         cached[dev] = n;
     }
     return cached[dev];
@@ -54,28 +54,7 @@ const char* zk_last_error(void) { return g_last_error.c_str(); }
 int64_t zk_launch_count(void) { return g_launches.load(); }
 int zk_set_fast_math(int on) { return g_fast_math.exchange(on ? 1 : 0); }
 int zk_set_fused_layers(int on) { return g_fused.exchange(on ? 1 : 0); }
-int zk_set_wide_min_hidden(int h) { return g_wide_min_h.exchange(h); }
-int zk_set_dual_tiles(int on) { return g_dual.exchange(on ? 1 : 0); }
 static thread_local cudaStream_t g_pack_stream = nullptr;
-void zk_debug_timeline(long long* device_buffer) { zk::g_timeline = device_buffer; }
-int zk_debug_wide_schedule(int n_linear, const int* dims, const uint8_t* const* masks_host, int univariate, int bins,
-                           int features, int context, uint32_t* out_items, int max_items, uint32_t* out_rd_mask,
-                           int* out_perm) {
-    return zk::wide_schedule_host(n_linear, dims, masks_host, univariate, bins, features, context, out_items, max_items,
-                                  out_rd_mask, out_perm);
-}
-int zk_debug_dual_schedule(int n_linear, const int* dims, const uint8_t* const* masks_host, int univariate, int bins,
-                           int features, int context, uint32_t* out_items, int max_items, uint32_t* out_rd_mask,
-                           int* out_perm) {
-    return zk::dual_schedule_host(n_linear, dims, masks_host, univariate, bins, features, context, out_items, max_items,
-                                  out_rd_mask, out_perm);
-}
-int zk_debug_watchdog_read(uint32_t* out, int n_words) {
-    if (!zk::g_watch_host || !out || n_words <= 0) return 0;
-    const int n = n_words < 1024 ? n_words : 1024;
-    for (int i = 0; i < n; ++i) out[i] = ((volatile uint32_t*)zk::g_watch_host)[i];
-    return n;
-}
 
 zk_status zk_device_info(int* sm, int* major, int* minor) {
     int dev = 0;
@@ -464,8 +443,8 @@ int zk_layer_fused_info(const zk_layer* l, double* out) {
     if (!pk || l->circ || !fused_layer_supported(m, l->uni, l->K, l->D, l->C)) return 0;
     const int kind = fused_layer_kind(m, l->uni, l->K, l->D, l->C);
     out[0] = kind;
-    out[1] = kind == 3 ? pk->dual.n_items : (kind == 2 ? pk->wide.n_items : pk->fused.n_items);
-    out[2] = kind == 3 ? pk->dual.issued_macs_per_row : (kind == 2 ? pk->wide.issued_macs_per_row : pk->fused.issued_macs_per_row);
+    out[1] = pk->fused.n_items;
+    out[2] = pk->fused.issued_macs_per_row;
     return kind;
 }
 
@@ -1037,10 +1016,9 @@ zk_status get_pipe(HostPipe** out) {
 
 }  // extern "C"
 
-/* Row chunks of the host pipeline.  The H2D copies run ahead of the compute (47 GB/s against ~30 GB/s of
-   input consumed by cfg2, less for every heavier flow), so a call costs copy(first chunk) + compute(all) +
-   a per-launch ramp per chunk: the first chunk is ONE wave of the persistent kernels (a wave = SMs/2 CTA pairs x
-   512 rows; chunks are whole waves, a 3.46-wave chunk runs as 4), the later ones grow by <= 1.7x — with two
+/* Row chunks of the host pipeline.  The H2D copies run ahead of the compute, so a call costs copy(first chunk) + compute(all) +
+   a per-launch ramp per chunk: the first chunk is ONE wave of the persistent kernels (a wave = one 64-row tile of the
+   fused layer kernel per SM; chunks are whole waves, a 3.46-wave chunk runs as 4), the later ones grow by <= 1.7x — with two
    staging slots the copy of chunk k starts when chunk k-2 is done and has to finish within the compute of
    chunk k-1 — up to `max_chunk` (what the workspace holds).  Small batches: eight equal chunks as before. */
 std::vector<int64_t> host_chunk_plan(int64_t B, int64_t wave, int64_t max_chunk) {
@@ -1074,7 +1052,7 @@ extern "C" {
 
 size_t zk_flow_host_workspace_bytes(const zk_flow_desc* f, int64_t B) {
     if (!f || B <= 0) return 1024;
-    const int64_t wave = (int64_t)(sm_count() / 2) * 512;
+    const int64_t wave = (int64_t)sm_count() * 64;
     int64_t big = 0;
     for (int64_t n : host_chunk_plan(B, wave, B)) big = std::max(big, n);
     return host_pipe_need(f, big) + 4096;
@@ -1106,7 +1084,7 @@ zk_status zk_flow_log_prob_host(const zk_flow_desc* f, const float* xh, int64_t 
     const size_t stage_row = (size_t)(D + (bc ? 0 : C) + 1) * 4;
     // chunk plan (host_chunk_plan): the step's time is the FIRST chunk's copy plus the compute of all of them,
     // so the first chunk is one wave and the later ones grow; bounded by the workspace
-    const int64_t wave = (int64_t)(sm_count() / 2) * 512;
+    const int64_t wave = (int64_t)sm_count() * 64;
     auto need = [&](int64_t n) { return host_pipe_need(f, n); };
     int64_t Bmax = B;
     while (Bmax > 1 && need(Bmax) > ws_bytes) Bmax = (Bmax > wave) ? std::max<int64_t>(wave, (Bmax / 2 / wave) * wave) : (Bmax + 1) / 2;

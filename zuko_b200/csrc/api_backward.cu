@@ -10,7 +10,7 @@
 //                        g = (g W_i) * [h_{i-1} > 0] linear_fp32_kernel on W_i^T + relu_gate_kernel
 //   gx = gx_direct + g[:, :D];  gc += g[:, D:]       input_grad_kernel
 // The flow-level call recomputes the forward chain z_0..z_T with the production forward kernels
-// (fused tcgen05 layer kernel where it applies), then walks the layers in reverse.
+// (fused layer kernel where it applies), then walks the layers in reverse.
 
 #include <mutex>
 
@@ -148,9 +148,9 @@ zk_status mlp_backward(const zk_mlp* m, const MlpBwdBufs& b, int64_t B, bool wan
 
 
 // ---------------------------------------------------------------------------
-// conditioner backward on the tensor cores (handles packed for tcgen05): every GEMM-shaped piece —
+// conditioner backward on the tensor cores (handles packed for wgmma): every GEMM-shaped piece —
 // forward recompute with saved activations, dgrad, wgrad — is linear_tc_kernel (split-bf16, fp32
-// accumulation in TMEM); see the block comment at the end of mlp_tcgen05.cu.
+// accumulation); see the block comment at the end of mlp_tcgen05.cu.
 // ---------------------------------------------------------------------------
 struct TcBwdPlan {
     int n = 0;
@@ -169,8 +169,8 @@ TcBwdPlan tc_plan(const zk_mlp* m, int64_t B) {
     for (int i = 0; i < p.n; ++i) {
         const int N = m->dims[i + 1], K = m->dims[i];
         const int sm = (N + 127) / 128 * 128;
-        const int64_t tiles = (int64_t)(sm / 128) * ((K + 255) / 256);
-        int64_t S = ceil_div(2 * 148, tiles);
+        const int64_t tiles = (int64_t)(sm / 128) * ((K + 127) / 128);
+        int64_t S = ceil_div(2 * sm_count(), tiles);
         S = std::max<int64_t>(1, std::min<int64_t>(S, B / 512));
         const int Bs = pad64((int)ceil_div(B, S));
         p.S.push_back((int)S);
@@ -260,7 +260,7 @@ zk_status tc_mlp_backward(const zk_mlp* m, const TcBwdPlan& p, const TcBwdBufs& 
             else ZK_TRY(launch_transpose_planes(g, B, p.Kp[i + 1], S, sm, Bs, b.gT, st));
             ZK_TRY(launch_transpose_planes(b.P[i], B, p.Kp[i], S, p.Kp[i], Bs, b.aT, st));
             CUtensorMap mapAT;
-            ZK_TRY(make_plane_map(&mapAT, b.aT, (int64_t)S * p.Kp[i], Bs, 256));
+            ZK_TRY(make_plane_map(&mapAT, b.aT, (int64_t)S * p.Kp[i], Bs, 128));
             TcGemmArgs w;
             w.a_planes = b.gT; w.M = (int64_t)S * sm; w.Kp = Bs; w.mapW = &mapAT; w.N = K;
             w.out_f32 = b.partial; w.ldo = K; w.slice_m = sm; w.w_slice_rows = p.Kp[i]; w.n_terms = pk->n_terms;

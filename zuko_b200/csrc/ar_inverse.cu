@@ -83,10 +83,14 @@ struct InvParams {
     const float* base_loc; const float* base_scale;
 };
 
+// two fp32 FMAs on a pair (fmaf rounding)
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+
 // acc[j][.] += sum_{k < K} state[k][sample j] * w[k][.]  over NT 8-row tiles stored k-major
-// ([k][NT * 8] weights): one state load per k feeds 8 NT FMAs, issued as packed FFMA2 (two fp32 FMAs
-// per instruction, same rounding as fmaf) — the loop is bound by shared-memory wavefronts and issue
-// slots, not by the FMA pipe.  The weights are read by every lane from the same address (broadcast).
+// ([k][NT * 8] weights): one state load per k feeds 8 NT FMAs.  The weights are read by every lane
+// from the same address (broadcast).
 template <int R, int NT>
 __device__ __forceinline__ void tile_dot(const float* __restrict__ w, const float* __restrict__ st, int K, int S, int T,
                                          float2 (&acc)[R][NT * 4]) {
@@ -103,8 +107,8 @@ __device__ __forceinline__ void tile_dot(const float* __restrict__ w, const floa
             const float4 wv = *reinterpret_cast<const float4*>(w + k * (NT * TILE) + 4 * q);
 #pragma unroll
             for (int j = 0; j < R; ++j) {
-                acc[j][2 * q] = __ffma2_rn(sv[j], make_float2(wv.x, wv.y), acc[j][2 * q]);
-                acc[j][2 * q + 1] = __ffma2_rn(sv[j], make_float2(wv.z, wv.w), acc[j][2 * q + 1]);
+                acc[j][2 * q] = fma2(sv[j], make_float2(wv.x, wv.y), acc[j][2 * q]);
+                acc[j][2 * q + 1] = fma2(sv[j], make_float2(wv.z, wv.w), acc[j][2 * q + 1]);
             }
         }
     }
@@ -210,7 +214,7 @@ __global__ void __launch_bounds__(256) ar_inverse_kernel(const InvParams p) {
 #pragma unroll
                     for (int j = 0; j < R; ++j) {
                         const float sv = Sl[k * S + j * T];
-                        acc[j] = __ffma2_rn(make_float2(sv, sv), wv, acc[j]);
+                        acc[j] = fma2(make_float2(sv, sv), wv, acc[j]);
                     }
                 }
                 wp += ((K + 1) * 2 + 3) & ~3;
@@ -325,7 +329,7 @@ zk_status launch_inv_t(const InvParams& p, bool fast, int R, int grid, int T, si
 }
 
 // threads per CTA, samples per thread and shared memory for a pack.  ZK_INV_GEOM=TxR overrides the
-// choice (experiments); the default is what measured fastest on cfg4.
+// choice (experiments); the default has not been re-tuned since the port to sm_90a.
 bool inv_geometry(const ArInvPack* pk, int* threads, int* per_thread, size_t* smem) {
     const size_t per_sample = (size_t)pk->state_floats * 4;
     const size_t wbytes = (size_t)pk->max_step_words * 4 + 16;

@@ -2,7 +2,7 @@
 //
 // First correct version of SURVEY §8(f) rank 1: plain fp32 CUDA-core kernels with fixed-order
 // (deterministic) reductions.  The three GEMM-shaped pieces — forward recompute, dgrad, wgrad —
-// run on fp32 FMA here; moving them to tcgen05 split-bf16 like the forward path is the next step.
+// run on fp32 FMA here; moving them to tensor-core split-bf16 like the forward path is the next step.
 
 #include <algorithm>
 
@@ -288,7 +288,7 @@ __global__ void transpose_kernel(const float* in, int N, int K, float* out) {
 
 int wgrad_slices_max(int N, int K) {
     const int64_t tiles = ceil_div(N, WO) * ceil_div(K, WI);
-    int64_t S = ceil_div(8 * 148, tiles);
+    int64_t S = ceil_div(8 * sm_count(), tiles);
     if (S > 64) S = 64;
     if (S < 1) S = 1;
     while (S > 1 && S * (int64_t)N * K * 4 > ((int64_t)256 << 20)) S /= 2;

@@ -72,9 +72,9 @@ ZK_HD void sc_parts(float v, float a, float& u, float& d) {
 //   gx  : dL/dx (direct dependence only), gp : dL/dp (P values; may alias p)
 // The softmax numerators / soft-clip derivatives of the 2K width / height parameters are recomputed
 // in each of the three sweeps (1 reciprocal + 1 exp per parameter and sweep).  Keeping them in
-// registers instead (kCacheNumerators) was measured SLOWER on B200: 92 instead of 64 registers per
-// thread at K = 8 halves the resident warps of this latency-bound kernel (1.04 ms vs 0.62 ms per
-// 2^18 x 16 pairs); the code path is kept for reference, both give bit-identical results.
+// registers instead (kCacheNumerators) costs registers (92 instead of 64 per thread at K = 8), which
+// halves the resident warps of this latency-bound kernel; the code path is kept for reference, both
+// give bit-identical results.
 constexpr bool kCacheNumerators = false;
 
 template <int KT_, bool FAST = false>

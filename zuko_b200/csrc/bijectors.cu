@@ -1,4 +1,4 @@
-// zuko_b200 — fused element-wise bijector kernels for sm_100a.
+// zuko_b200 — fused element-wise bijector kernels for sm_90a.
 //
 // uni_kernel: one pass per flow layer over (B, D) with per-sample parameters
 //   phi (B, D, P):  x, phi  ->  y, sum_d log|dy/dx|  (+ optional DiagNormal log-prob)

@@ -1,4 +1,4 @@
-// zuko_b200 — shared host/device helpers (sm_100a only).
+// zuko_b200 — shared host/device helpers (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -98,7 +98,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // non-blocking probe (try_wait may suspend the thread for a system-dependent time before it
-// reports failure — thousands of cycles on B200 — so look-ahead polls must use test_wait)
+// reports failure — possibly thousands of cycles — so look-ahead polls must use test_wait)
 __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
     uint32_t done;
     asm volatile(

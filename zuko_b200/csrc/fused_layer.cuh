@@ -25,30 +25,13 @@ struct FusedLayerArgs {
 
 // true when the autoregressive layer (conditioner `m`, univariate, D, C) can run as ONE kernel
 bool fused_layer_supported(const zk_mlp* m, int univariate, int bins, int D, int C);
-// which kernel: 0 none, 1 one CTA per tile (fused_layer.cu), 2 CTA pairs (fused_wide.cu), 3 CTA pairs with two sub-tiles (fused_dual.cu)
+// which kernel: 0 none, 1 the fused layer kernel (fused_layer.cu)
 int fused_layer_kind(const zk_mlp* m, int univariate, int bins, int D, int C);
 // Builds the fused kernel's weight pack for this conditioner (degree-sorted hidden units, zero-tile
 // map); `mask_dev` are the DEVICE mask pointers of zk_mlp_desc (may be null = dense).  No-op when
 // the shape is not supported by the fused kernel.
 zk_status fused_layer_prepare(zk_mlp* m, const uint8_t* const* mask_dev, int univariate, int bins, int D, int C);
-// ---- wide variant (fused_wide.cu): hidden width 384 / 512 on CTA pairs (cta_group::2) ----
-// shape test only; the layer runs fused once fused_wide_prepare built a schedule that passed its dry run
-bool fused_wide_shape(const zk_mlp* m, int univariate, int bins, int D, int C);
-zk_status fused_wide_prepare(zk_mlp* m, const uint8_t* const* mask_dev, int univariate, int bins, int D, int C);
-zk_status launch_fused_wide(const zk_mlp* m, const FusedLayerArgs& a, cudaStream_t stream);
-int wide_schedule_host(int n_linear, const int* dims, const uint8_t* const* masks_host, int univariate, int bins, int D,
-                       int C, uint32_t* out_items, int max_items, uint32_t* out_rd_mask, int* out_perm);
-// ---- dual-tile variant (fused_dual.cu): hidden width 128 / 256, two sub-tiles in flight per CTA ----
-bool fused_dual_shape(const zk_mlp* m, int univariate, int bins, int D, int C);
-zk_status fused_dual_prepare(zk_mlp* m, const uint8_t* const* mask_dev, int univariate, int bins, int D, int C);
-zk_status launch_fused_dual(const zk_mlp* m, const FusedLayerArgs& a, cudaStream_t stream);
-int dual_schedule_host(int n_linear, const int* dims, const uint8_t* const* masks_host, int univariate, int bins, int D,
-                       int C, uint32_t* out_items, int max_items, uint32_t* out_rd_mask, int* out_perm);
-extern std::atomic<int> g_dual;
-extern std::atomic<int> g_wide_min_h;
-extern uint32_t* g_watch_host;  // watchdog report buffer of the wide kernel (pinned host memory) or null
 zk_status fused_refresh(zk_mlp* m, cudaStream_t stream);  // weights changed in place: re-split into the fused packs
-extern long long* g_timeline;  // device buffer of >= 256 stamps, or null (zk_debug_timeline)
 zk_status launch_fused_layer(const zk_mlp* m, const FusedLayerArgs& a, cudaStream_t stream);
 
 }  // namespace zk

@@ -19,7 +19,7 @@ struct zk_mlp {
     bool bwd_dirty = false;        // weights refreshed since wt / the backward planes were built
     int gemm_mode = ZK_GEMM_FP32;  // resolved path
     int max_hidden = 0;
-    // tcgen05 path: packed bf16 hi/lo weights (owned), see mlp_tcgen05.cu
+    // tensor-core path: packed bf16 hi/lo weights (owned), see mlp_tcgen05.cu
     void* tc = nullptr;
 };
 

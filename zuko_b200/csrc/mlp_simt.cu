@@ -2,7 +2,7 @@
 //
 // relu?(A W^T + b) with fp32 FMA accumulation, any shape.  This is the reference-order
 // path (ZK_GEMM_FP32): it serves shapes too small for a tensor-core tile (BASELINE cfg1:
-// 4 -> 32 -> 32 -> 8) and validates the tcgen05 split-bf16 path (mlp_tcgen05.cu), which is
+// 4 -> 32 -> 32 -> 8) and validates the tensor-core split-bf16 path (mlp_tcgen05.cu), which is
 // the production path for the large conditioners.  Restates zuko/nn.py:217-218 with the
 // mask multiplication hoisted to pack time.
 

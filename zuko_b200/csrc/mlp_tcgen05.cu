@@ -1,28 +1,27 @@
-// zuko_b200 — conditioner GEMMs on the 5th-generation tensor cores (tcgen05, sm_100a).
+// zuko_b200 — conditioner GEMMs on the Hopper tensor cores (wgmma, sm_90a).
 //
 // One linear layer  C[M, N] = act(A[M, K] W[N, K]^T + b)  of MaskedMLP / MLP
 // (zuko/nn.py:217-218 with the mask folded into W at pack time) as a persistent,
-// warp-specialised kernel:
+// warp-specialised kernel over 128 x 128 output tiles:
 //
-//   warp 0   TMA producer : cp.async.bulk.tensor (128B-swizzled boxes) of the A and W tiles
-//                           into a shared-memory ring, completion on mbarriers (complete_tx)
-//   warp 1   MMA issuer   : one elected lane issues tcgen05.mma.cta_group::1.kind::f16
-//                           (M = 128, N <= 256, K = 16 per instruction), accumulators in TMEM,
-//                           tcgen05.commit releases the smem slot / publishes the accumulator
-//   warp 2   TMEM allocator (tcgen05.alloc / dealloc, 512 columns = 2 accumulator stages)
-//   warps 4-7 epilogue    : tcgen05.ld (32x32b: thread = sample row) -> bias, ReLU ->
-//                           either bf16 hi/lo planes for the next layer or fp32 phi
+//   warpgroup 0   TMA producer : one thread issues cp.async.bulk.tensor (128B-swizzled boxes) of the
+//                                A and W tiles into a shared-memory ring, completion on mbarriers
+//   warpgroups 1-2 consumers   : warpgroup g owns rows [64 (g - 1), 64 g) of the tile; it issues
+//                                wgmma.mma_async m64n64k16 (both operands in shared memory, fp32
+//                                accumulators in registers), releases the ring slot, and runs the
+//                                epilogue (bias, activation -> fp32 phi or bf16 hi/lo planes for the
+//                                next layer) straight from the accumulator registers
 //
 // Precision: fp32 inputs are carried as TWO bf16 planes (hi = rn(v), lo = rn(v - hi)) and the
-// product is formed as  A_hi W_hi + A_hi W_lo + A_lo W_hi  with fp32 accumulation in TMEM
+// product is formed as  A_hi W_hi + A_hi W_lo + A_lo W_hi  with fp32 accumulation
 // (ZK_GEMM_BF16X3).  A single bf16 MMA misses the 1e-5 parity bar of BASELINE.json (1.4e-4 on
-// config 2, SURVEY §7.4-1); the 3-MMA split meets it (1.1e-6).  ZK_GEMM_BF16X1 keeps only the
-// first term (fast, inexact, opt-in).
+// config 2, SURVEY §7.4-1); the 3-MMA split meets it.  ZK_GEMM_BF16X1 keeps only the first term
+// (fast, inexact, opt-in).
 //
 // Operand layout in HBM: activations act[plane][M][Kp] and weights w[plane][N][Kp], bf16,
 // K contiguous ("K-major"), Kp = K rounded up to 64 with zero padding.  A TMA box of
 // (64 x rows) bf16 lands in shared memory as rows of 128 bytes with the 128B swizzle, which is
-// the canonical K-major SWIZZLE_128B UMMA operand layout (8-row groups 1024 B apart).
+// the K-major SWIZZLE_128B wgmma operand layout (8-row groups 1024 B apart).
 
 #include "activations.cuh"
 #include "mlp_tcgen05.cuh"
@@ -32,18 +31,15 @@ namespace zk {
 
 namespace {
 
-constexpr int BM = 128;        // rows per tile = TMEM lanes
-constexpr int BN = 256;        // max accumulator columns per tile
+constexpr int BM = 128;        // rows per tile (two warpgroups of 64)
+constexpr int BN = 128;        // output columns per tile (two 64-wide MMA column blocks)
 constexpr int BK = 64;         // bf16 per K block = one 128-byte swizzle row
-constexpr int UMMA_K = 16;     // K per tcgen05.mma (bf16)
-constexpr int STAGES = 2;      // shared-memory ring depth
-constexpr int ACC_STAGES = 2;  // TMEM accumulator stages (2 x 256 columns = all of TMEM)
-constexpr int kThreads = 256;
-constexpr int kEpiWarp0 = 4;
+constexpr int STAGES = 3;      // shared-memory ring depth
+constexpr int kThreads = 384;  // producer warpgroup + two consumer warpgroups
 
 constexpr uint32_t A_TILE_BYTES = BM * BK * 2;  // 16 KB per plane
-constexpr uint32_t W_TILE_BYTES = BN * BK * 2;  // 32 KB per plane
-constexpr uint32_t STAGE_BYTES = 2 * A_TILE_BYTES + 2 * W_TILE_BYTES;  // 96 KB
+constexpr uint32_t W_TILE_BYTES = BN * BK * 2;  // 16 KB per plane
+constexpr uint32_t STAGE_BYTES = 2 * A_TILE_BYTES + 2 * W_TILE_BYTES;  // 64 KB
 constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 
 struct TcParams {
@@ -67,13 +63,15 @@ struct TcParams {
     int w_slice_rows;
 };
 
+// relu(bf16 v) > 0 test on the raw bits: positive and not zero
+__device__ __forceinline__ bool bf16_positive(uint32_t b) { return (b & 0x7fffu) != 0u && (b & 0x8000u) == 0u; }
+
 // ---------------------------------------------------------------------------
 // the GEMM kernel
 // ---------------------------------------------------------------------------
 // GENERAL_ACT = false: epilogue activation none / ReLU only (the hot instantiation — every BASELINE config);
-// true: any ZK_ACT_* through act_apply().  Two instantiations because the general switch, inlined into
-// the 32-wide unrolled epilogue, grows the kernel from 2.8 k to 16 k SASS lines and slowed the ReLU
-// path ~2x (instruction cache) when it was a run-time branch of one kernel.
+// true: any ZK_ACT_* through act_apply() and the residual input.  Two instantiations keep the general
+// switch out of the hot epilogue.
 template <bool GENERAL_ACT>
 __global__ void __launch_bounds__(kThreads, 1)
 linear_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW,
@@ -82,14 +80,10 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     // 1024-byte alignment: SWIZZLE_128B atoms are 8 rows x 128 B
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t* bars = (uint64_t*)(smem + (size_t)STAGES * STAGE_BYTES);
-    uint64_t* full_bar = bars;                       // [STAGES]   TMA -> MMA
-    uint64_t* empty_bar = bars + STAGES;             // [STAGES]   MMA -> TMA
-    uint64_t* acc_full = bars + 2 * STAGES;          // [ACC_STAGES] MMA -> epilogue
-    uint64_t* acc_empty = acc_full + ACC_STAGES;     // [ACC_STAGES] epilogue -> MMA
-    uint32_t* tmem_slot = (uint32_t*)(acc_empty + ACC_STAGES);
+    uint64_t* full_bar = bars;            // [STAGES]   TMA -> consumers
+    uint64_t* empty_bar = bars + STAGES;  // [STAGES]   consumers -> TMA (one arrival per consumer warpgroup)
 
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     const int m_tiles = (p.M + BM - 1) / BM;
     const int total_tiles = m_tiles * p.n_chunks;
     const int k_blocks = p.Kp / BK;
@@ -97,28 +91,15 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int a = 0; a < ACC_STAGES; ++a) {
-            mbar_init(&acc_full[a], 1);
-            mbar_init(&acc_empty[a], 128);
+            mbar_init(&empty_bar[s], 2);
         }
         fence_mbar_init();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, ACC_STAGES * BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    // A 512-column allocation is the whole tensor memory, so its base is always lane 0 / column 0.
-    // Using the literal keeps every tcgen05 address in uniform registers: with the address read
-    // back from shared memory ptxas wrapped each UTCHMMA in an ELECT / R2UR.BROADCAST waterfall
-    // loop (~110 cycles per MMA instead of 64).
-    if (*tmem_slot != 0u) __trap();
-    constexpr uint32_t tmem_base = 0u;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ================= TMA producer =================
-        if (lane == 0) {
+        if (threadIdx.x == 0) {
             const uint32_t bytes = (p.n_terms == 3) ? STAGE_BYTES : (A_TILE_BYTES + W_TILE_BYTES);
             int stage = 0;
             uint32_t phase = 0;
@@ -141,154 +122,94 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        // whole warp converged, one elected lane issues (keeps every tcgen05 operand in uniform
-        // registers; see fused_layer.cu)
-        int stage = 0, acc = 0;
-        uint32_t phase = 0, acc_phase = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-            const int n0 = (t % p.n_chunks) * BN;
-            int n_sz = p.N - n0;                       // columns of this chunk
-            n_sz = n_sz > BN ? BN : ((n_sz + 15) & ~15);  // UMMA N: multiple of 16 (M = 128)
-            const uint32_t idesc = umma_idesc_bf16(BM, n_sz);
-            mbar_wait(&acc_empty[acc], acc_phase ^ 1);
-            const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-            for (int kb = 0; kb < k_blocks; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                const uint32_t sbase = smem_u32(smem) + (uint32_t)stage * STAGE_BYTES;
-                const uint64_t da_hi = umma_desc_k_sw128(sbase), da_lo = umma_desc_k_sw128(sbase + A_TILE_BYTES);
-                const uint64_t dw_hi = umma_desc_k_sw128(sbase + 2 * A_TILE_BYTES);
-                const uint64_t dw_lo = umma_desc_k_sw128(sbase + 2 * A_TILE_BYTES + W_TILE_BYTES);
-                if (elect_one()) {
+        return;
+    }
+
+    // ================= consumers: MMA + epilogue =================
+    const int h = wg - 1;                 // row half of the tile
+    const int tid = threadIdx.x & 127;
+    const int w = tid >> 5, lane = tid & 31;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+        const int m0 = (t / p.n_chunks) * BM;
+        const int n0 = (t % p.n_chunks) * BN;
+        const int n_sz = min(BN, p.N - n0);  // real columns of this tile (> 0)
+        float acc[2][32];
 #pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {
-                        umma_bf16(d_tmem, umma_desc_advance(da_hi, k), umma_desc_advance(dw_hi, k), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                        if (p.n_terms == 3) {
-                            umma_bf16(d_tmem, umma_desc_advance(da_hi, k), umma_desc_advance(dw_lo, k), idesc, 1u);
-                            umma_bf16(d_tmem, umma_desc_advance(da_lo, k), umma_desc_advance(dw_hi, k), idesc, 1u);
-                        }
-                    }
-                    umma_commit(&empty_bar[stage]);  // slot free once these MMAs have read it
-                    if (kb == k_blocks - 1) umma_commit(&acc_full[acc]);  // accumulator complete
-                }
-                __syncwarp();
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-            if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
+        for (int c = 0; c < 2; ++c)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+        for (int kb = 0; kb < k_blocks; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sbase = smem_u32(smem) + (uint32_t)stage * STAGE_BYTES;
+            const uint32_t a_hi = sbase + (uint32_t)h * (A_TILE_BYTES / 2), a_lo = a_hi + A_TILE_BYTES;
+            const uint32_t w_hi = sbase + 2 * A_TILE_BYTES, w_lo = w_hi + W_TILE_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int c = 0; c < 2; ++c)
+                if (c * 64 < n_sz)
+                    wgmma_kblock(acc[c], a_hi, a_lo, w_hi + (uint32_t)c * (W_TILE_BYTES / 2), w_lo + (uint32_t)c * (W_TILE_BYTES / 2),
+                                 p.n_terms);
+            wgmma_commit();
+            wgmma_wait0();
+            acc_fence(acc[0]);
+            acc_fence(acc[1]);
+            if (tid == 0) mbar_arrive(&empty_bar[stage]);  // slot free: this warpgroup's MMAs have read it
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-    } else if (warp >= kEpiWarp0) {
-        // ================= epilogue =================
-        const int q = warp & 3;  // TMEM lane quadrant this warp may access
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-            const int m0 = (t / p.n_chunks) * BM;
-            const int n0 = (t % p.n_chunks) * BN;
-            const int row = m0 + q * 32 + lane;
-            const bool row_ok = row < p.M;
-            int n_sz = p.N - n0;
-            n_sz = n_sz > BN ? BN : n_sz;                    // real columns in this chunk
-            const int n_pad = (p.out_f32 != nullptr) ? n_sz  // fp32 phi: real columns only
-                                                     : min(BN, p.Np - n0);  // planes: up to the padded width
-            mbar_wait(&acc_full[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN);
-            for (int c0 = 0; c0 < n_pad; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld_32x32b_x32(t_row + (uint32_t)c0, r);
-                tmem_ld_wait();
-                float v[32];
+        // ---- epilogue straight from the accumulator registers ----
+        const int r_base = m0 + h * 64 + w * 16 + (lane >> 2);
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int n = n0 + c0 + j;
-                    float f = __uint_as_float(r[j]) + ((p.bias != nullptr && n < p.N) ? __ldg(p.bias + n) : 0.f);
-                    if constexpr (GENERAL_ACT) {
-                        if (p.relu == 1) f = fmaxf(f, 0.f);
-                        else if (p.relu > 1) f = act_apply(f, p.relu);
-                    } else {
-                        if (p.relu) f = fmaxf(f, 0.f);
-                    }
-                    v[j] = (n < p.N) ? f : 0.f;  // padded columns feed the next layer as exact zeros
-                }
-                if (!row_ok) continue;
-                if (p.out_f32 != nullptr) {
-                    float* dst = p.out_f32 + (int64_t)row * p.ldo + n0 + c0;
-                    const int lim = n_sz - c0;  // > 0
-                    if (lim >= 32 && (((uintptr_t)dst) & 15) == 0) {
+        for (int c = 0; c < 2; ++c) {
 #pragma unroll
-                        for (int j = 0; j < 32; j += 4)
-                            *reinterpret_cast<float4*>(dst + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                    } else {
+            for (int i = 0; i < 8; ++i) {
+                const int n = n0 + c * 64 + 8 * i + 2 * (lane & 3);  // first of the thread's two columns
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (j < lim) dst[j] = v[j];
-                    }
-                } else {
-                    if (p.gate != nullptr) {  // d relu: zero where the forward activation was not positive
-                        const uint4* gp = reinterpret_cast<const uint4*>(p.gate + (int64_t)row * p.Np + n0 + c0);
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int row = r_base + 8 * hh;
+                    if (row >= p.M) continue;
+                    float v[2];
 #pragma unroll
-                        for (int q4 = 0; q4 < 4; ++q4) {
-                            const uint4 gv = __ldg(gp + q4);
-                            const uint32_t w4[4] = {gv.x, gv.y, gv.z, gv.w};
-#pragma unroll
-                            for (int u = 0; u < 4; ++u) {
-                                const uint32_t b0 = w4[u] & 0xffffu, b1 = w4[u] >> 16;
-                                const int j = q4 * 8 + u * 2;
-                                if (!((b0 & 0x7fffu) != 0u && (b0 & 0x8000u) == 0u)) v[j] = 0.f;
-                                if (!((b1 & 0x7fffu) != 0u && (b1 & 0x8000u) == 0u)) v[j + 1] = 0.f;
-                            }
+                    for (int e = 0; e < 2; ++e) {
+                        float f = acc[c][4 * i + 2 * hh + e] + ((p.bias != nullptr && n + e < p.N) ? __ldg(p.bias + n + e) : 0.f);
+                        if constexpr (GENERAL_ACT) {
+                            if (p.relu == 1) f = fmaxf(f, 0.f);
+                            else if (p.relu > 1) f = act_apply(f, p.relu);
+                        } else {
+                            if (p.relu) f = fmaxf(f, 0.f);
                         }
+                        v[e] = (n + e < p.N) ? f : 0.f;  // padded columns feed the next layer as exact zeros
+                    }
+                    if (p.out_f32 != nullptr) {
+                        float* dst = p.out_f32 + (int64_t)row * p.ldo + n;
+                        if (n < p.N) dst[0] = v[0];
+                        if (n + 1 < p.N) dst[1] = v[1];
+                        continue;
+                    }
+                    if (n >= p.Np) continue;  // Np is even: the pair is in range together
+                    const int64_t off = (int64_t)row * p.Np + n;
+                    if (p.gate != nullptr) {  // d relu: zero where the forward activation was not positive
+                        const uint32_t gv = __ldg(reinterpret_cast<const unsigned int*>(p.gate + off));
+                        if (!bf16_positive(gv & 0xffffu)) v[0] = 0.f;
+                        if (!bf16_positive(gv >> 16)) v[1] = 0.f;
                     }
                     if constexpr (GENERAL_ACT) {
-                        if (p.res != nullptr) {
-                            const uint4* rh = reinterpret_cast<const uint4*>(p.res + (int64_t)row * p.Np + n0 + c0);
-                            const uint4* rl = reinterpret_cast<const uint4*>(p.res + (int64_t)p.M * p.Np + (int64_t)row * p.Np + n0 + c0);
-#pragma unroll
-                            for (int q4 = 0; q4 < 4; ++q4) {
-                                const uint4 a = rh[q4], b = rl[q4];  // plain loads: the planes may be the ones written below
-                                const uint32_t ah[4] = {a.x, a.y, a.z, a.w}, al[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-                                for (int u = 0; u < 4; ++u) {
-                                    const int j = q4 * 8 + u * 2;
-                                    v[j] += __uint_as_float(ah[u] << 16) + __uint_as_float(al[u] << 16);
-                                    v[j + 1] += __uint_as_float(ah[u] & 0xffff0000u) + __uint_as_float(al[u] & 0xffff0000u);
-                                }
-                            }
+                        if (p.res != nullptr) {  // plain loads: the planes may be the ones written below
+                            const uint32_t a = *reinterpret_cast<const uint32_t*>(p.res + off);
+                            const uint32_t b = *reinterpret_cast<const uint32_t*>(p.res + (int64_t)p.M * p.Np + off);
+                            v[0] += __uint_as_float(a << 16) + __uint_as_float(b << 16);
+                            v[1] += __uint_as_float(a & 0xffff0000u) + __uint_as_float(b & 0xffff0000u);
                         }
                     }
                     // split into bf16 hi / lo planes (K-major operand of the next layer)
-                    __nv_bfloat16* hi = p.out_planes + (int64_t)row * p.Np + n0 + c0;
-                    __nv_bfloat16* lo = hi + (int64_t)p.M * p.Np;
-                    uint32_t ph[16], pl[16];
-#pragma unroll
-                    for (int j = 0; j < 32; j += 2) {
-                        const __nv_bfloat16 h0 = __float2bfloat16_rn(v[j]), h1 = __float2bfloat16_rn(v[j + 1]);
-                        const __nv_bfloat16 l0 = __float2bfloat16_rn(v[j] - __bfloat162float(h0));
-                        const __nv_bfloat16 l1 = __float2bfloat16_rn(v[j + 1] - __bfloat162float(h1));
-                        ph[j >> 1] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                        pl[j >> 1] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-                    }
-                    // Np is a multiple of 64 and c0 of 32 => 64-byte aligned 16-byte vector stores
-#pragma unroll
-                    for (int j = 0; j < 16; j += 4) {
-                        *reinterpret_cast<uint4*>(reinterpret_cast<uint32_t*>(hi) + j) = make_uint4(ph[j], ph[j + 1], ph[j + 2], ph[j + 3]);
-                        *reinterpret_cast<uint4*>(reinterpret_cast<uint32_t*>(lo) + j) = make_uint4(pl[j], pl[j + 1], pl[j + 2], pl[j + 3]);
-                    }
+                    uint32_t ph, pl;
+                    split2_bf16(v[0], v[1], ph, pl);
+                    *reinterpret_cast<uint32_t*>(p.out_planes + off) = ph;
+                    *reinterpret_cast<uint32_t*>(p.out_planes + (int64_t)p.M * p.Np + off) = pl;
                 }
             }
-            tc_fence_before();
-            mbar_arrive(&acc_empty[acc]);
-            if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, ACC_STAGES * BN);
     }
 }
 
@@ -384,9 +305,7 @@ void tc_destroy(zk_mlp* m) {
     for (auto* q : pk->fused.w) cudaFree(q);
     for (auto* q : pk->fused.bias) cudaFree(q);
     for (auto* q : pk->fused.dperm) cudaFree(q);
-    cudaFree(pk->fused.sched);
-    cudaFree(pk->wide.sched);
-    cudaFree(pk->dual.sched);
+    cudaFree(pk->fused.last_rows);
     delete pk;
     m->tc = nullptr;
 }
@@ -402,11 +321,11 @@ zk_status tc_pack(zk_mlp* m, int requested_mode) {
     int dev = 0, major = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess)
         return fail(ZK_ECUDA, "tc_pack: no CUDA device");
-    if (major != 10) eligible = false;  // tcgen05 exists on sm_100 only
+    if (major != 9) eligible = false;  // the wgmma kernels are built for sm_90a only
     if (!encode_fn()) eligible = false;
     if (!eligible) {
         if (requested_mode == ZK_GEMM_AUTO) return ZK_OK;
-        return fail(ZK_EUNSUPPORTED, "tcgen05 GEMM path unavailable (needs sm_100 and layer widths >= 64; widest is %d)", max_dim);
+        return fail(ZK_EUNSUPPORTED, "tensor-core GEMM path unavailable (needs sm_90 and layer widths >= 64; widest is %d)", max_dim);
     }
     TcPack* pk = new TcPack();
     pk->n_terms = (requested_mode == ZK_GEMM_BF16X1) ? 1 : 3;
@@ -425,8 +344,6 @@ zk_status tc_pack(zk_mlp* m, int requested_mode) {
         split_weight_kernel<<<(unsigned)ceil_div((int64_t)L.N * L.Kp, 256), 256, 0, 0>>>(m->w[i], L.N, L.K, L.Kp, L.w);
         ZK_TRY(check_launch("split_weight_kernel"));
         ZK_TRY(make_plane_map(&pk->layers.back().mapW, L.w, L.N, L.Kp, BN));
-        ZK_TRY(make_plane_map(&pk->layers.back().mapW128, L.w, L.N, L.Kp, 128));
-        ZK_TRY(make_plane_map(&pk->layers.back().mapW64, L.w, L.N, L.Kp, 64));
         if (i < m->n_linear - 1) pk->max_np = std::max(pk->max_np, pad64(L.N));
     }
     ZK_CUDA(cudaFuncSetAttribute(linear_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));

@@ -1,4 +1,4 @@
-// zuko_b200 — tcgen05 (5th-gen tensor core) conditioner path: interface.
+// zuko_b200 — tensor-core (wgmma) conditioner path: interface.
 #pragma once
 
 #include <cuda.h>
@@ -24,7 +24,7 @@ struct TcGemmArgs {
     const __nv_bfloat16* a_planes = nullptr;  // [2][M][Kp] bf16 hi / lo
     int64_t M = 0;
     int Kp = 0;
-    const CUtensorMap* mapW = nullptr;  // planes [2][rows][Kp], box (64 x 256 x 1)
+    const CUtensorMap* mapW = nullptr;  // planes [2][rows][Kp], box (64 x 128 x 1)
     int N = 0;                          // real output columns
     const float* bias = nullptr;
     int relu = 0;

@@ -1,4 +1,4 @@
-// zuko_b200 — tcgen05 / TMA / TMEM PTX wrappers and the packed-weight structures shared by the
+// zuko_b200 — wgmma / TMA PTX wrappers (sm_90a) and the packed-weight structures shared by the
 // per-layer GEMM kernel (mlp_tcgen05.cu) and the fused layer kernel (fused_layer.cu).
 #pragma once
 
@@ -23,136 +23,101 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
         : "memory");
 }
 
-// multicast variant: the box lands at the same CTA-relative offset in every CTA of `mask`, and each
-// destination CTA's mbarrier (same offset) receives the complete_tx
-__device__ __forceinline__ void tma_load_3d_mc(void* smem_dst, const CUtensorMap* map, uint64_t* bar,
-                                               int c0, int c1, int c2, uint16_t mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%3, %4, %5}], [%2], %6;"
-        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
-        : "memory");
-}
-// commit that arrives on the mbarrier at the same offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// one leader lane of a converged warp (PTX elect.sync); lets the single-thread tcgen05 / TMA issue
-// sit inside warp-uniform control flow so that its operands stay in uniform registers
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-        "elect.sync rx|px, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, px;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-// descriptor of the k-th 16-element K step inside a 64-wide swizzled K block: +32 bytes = +2 units
-__device__ __forceinline__ uint64_t umma_desc_advance(uint64_t desc, int k) { return desc + (uint64_t)(2 * k); }
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+// named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory descriptor, K-major, SWIZZLE_128B (cute::UMMA::SmemDescriptor):
+// wgmma shared-memory descriptor, K-major, SWIZZLE_128B (operand rows of 128 bytes, 8-row groups
+// 1024 B apart, 1024-byte aligned base):
 //   [0,14) start address >> 4 | [16,30) LBO >> 4 (unused for swizzled K-major, 1) |
-//   [32,46) SBO >> 4 = 1024 B between 8-row groups | [46,48) version = 1 | [61,64) layout = 2
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+//   [32,46) SBO >> 4 = 1024 B | [62,64) layout 1 = 128B swizzle
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// tcgen05 instruction descriptor (cute::UMMA::InstrDescriptor), kind::f16:
-//   [4,6) D format 1 = f32 | [7,10) A format 1 = bf16 | [10,13) B format 1 = bf16 |
-//   bit 15 / 16: A / B major 0 = K | [17,23) N >> 3 | [24,29) M >> 4
-__device__ __forceinline__ uint32_t umma_idesc_bf16(int m, int n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+// descriptor of the k-th 16-element K step inside a 64-wide swizzled K block: +32 bytes = +2 units
+__device__ __forceinline__ uint64_t gmma_desc_advance(uint64_t desc, int k) { return desc + (uint64_t)(2 * k); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void acc_fence(float (&d)[32]) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// D[64 x 64] += A[64 x 16] * B[64 x 16]^T (one warpgroup; bf16 inputs, fp32 accumulators in registers).
+// Accumulator layout (thread t of the warpgroup, w = t / 32, l = t % 32):
+//   d[4 i + 2 h + e] = D[16 w + l / 4 + 8 h][8 i + 2 (l % 4) + e]
+__device__ __forceinline__ void wgmma_m64n64k16_bf16(float (&d)[32], uint64_t desc_a, uint64_t desc_b) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(desc_a), "l"(desc_b));
+}
+
+// One 64-wide K block of the split-bf16 product on 64 x 64 tiles: hi*hi (+ hi*lo + lo*hi when n_terms == 3).
+// a_hi / a_lo / b_hi / b_lo: shared-memory addresses of 128B-swizzled K-major 64-row operand tiles.
+__device__ __forceinline__ void wgmma_kblock(float (&d)[32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                             int n_terms) {
+    const uint64_t dah = gmma_desc_sw128(a_hi), dal = gmma_desc_sw128(a_lo);
+    const uint64_t dbh = gmma_desc_sw128(b_hi), dbl = gmma_desc_sw128(b_lo);
+    if (n_terms == 3) {  // one branch outside the MMA sequence: no register hand-off between the MMAs
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            wgmma_m64n64k16_bf16(d, gmma_desc_advance(dah, k), gmma_desc_advance(dbh, k));
+            wgmma_m64n64k16_bf16(d, gmma_desc_advance(dah, k), gmma_desc_advance(dbl, k));
+            wgmma_m64n64k16_bf16(d, gmma_desc_advance(dal, k), gmma_desc_advance(dbh, k));
+        }
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n64k16_bf16(d, gmma_desc_advance(dah, k), gmma_desc_advance(dbh, k));
+    }
+}
+
+// byte offset of K element k (< 64) of row r inside a 128B-swizzled tile of 128-byte rows
+__device__ __forceinline__ uint32_t sw128_offset(int r, int k) {
+    return (uint32_t)r * 128u + ((((uint32_t)k >> 3) ^ ((uint32_t)r & 7u)) << 4) + (((uint32_t)k & 7u) << 1);
+}
 
 struct TcLayer {
     int N = 0, K = 0, Kp = 0;
     __nv_bfloat16* w = nullptr;  // [2][N][Kp] (owned)
-    CUtensorMap mapW;     // box (64 x 256 x 1): per-layer GEMM kernel
-    CUtensorMap mapW128;  // box (64 x 128 x 1)
-    CUtensorMap mapW64;   // box (64 x 64 x 1): fused layer kernel, one half per CTA of a pair (multicast)
+    CUtensorMap mapW;            // box (64 x 128 x 1): per-layer GEMM kernel
 };
 // weights as the fused layer kernel streams them: hidden units sorted by dependency degree (so
-// that the masked matrices are block lower-triangular) and the all-zero (chunk, K block) tiles
-// of every layer recorded so that their TMA loads and MMAs are skipped
+// that the masked matrices are block lower-triangular), the output layer's rows regrouped so that
+// every 64-row chunk holds whole dims, and the all-zero (chunk, K block) tiles of every layer
+// recorded so that their loads and MMAs are skipped
 struct FusedPack {
     bool ready = false;
     int uni = 0, bins = 0, D = 0, C = 0;
-    std::vector<__nv_bfloat16*> w;  // per layer [2][N][Kp], permuted (owned)
+    std::vector<__nv_bfloat16*> w;  // per layer [2][N][Kp], permuted (owned); output layer [2][n_last * 64][Kp]
     std::vector<float*> bias;       // per layer, permuted, padded (owned)
     std::vector<int*> dperm;        // per hidden layer: device copy of the degree permutation (owned; weight refresh)
+    int* last_rows = nullptr;       // device: output-layer row of every padded output row, -1 = zero row (owned)
+    int n_last = 0;                 // 64-row chunks of the output layer
     std::vector<CUtensorMap> map64; // box (64 x 64 x 1)
     uint8_t kbmask[8][128];         // [layer][chunk]: bit kb = K block kb has non-zero weights
-    uint32_t* sched = nullptr;      // device: MMA issue schedule of one tile, one entry per non-zero tile (owned)
-    int n_items = 0;
-    double issued_macs_per_row = 0;  // MACs the schedule issues per sample row (all split terms), bench bookkeeping
-};
-// the wide fused kernel's pack (fused_wide.cu): it shares FusedPack's permuted planes / biases
-// (fused.w, fused.bias) and adds its own tensor maps and issue schedule
-struct WidePack {
-    bool ready = false;
-    int uni = 0, bins = 0, D = 0, C = 0;
-    std::vector<CUtensorMap> maps;  // per layer: box (64 x 64 x 1) hidden, (64 x N_LAST/2 x 1) output layer
-    uint2* sched = nullptr;         // device: one entry per non-zero (layer, chunk, K block) tile (owned)
-    int n_items = 0;
-    uint8_t rd_mask[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // per layer: K blocks of the A operand the layer reads
-    double issued_macs_per_row = 0;  // MACs the schedule issues per sample row (all split terms)
+    double issued_macs_per_row = 0;  // MACs the kernel issues per sample row (all split terms), bench bookkeeping
+    int n_items = 0;                 // non-zero 64 x 64 weight tiles streamed per row tile
 };
 struct TcPack {
     std::vector<TcLayer> layers;
@@ -160,8 +125,6 @@ struct TcPack {
     int n_terms = 3;
     int max_np = 0;  // widest padded hidden activation
     FusedPack fused;
-    WidePack wide;
-    WidePack dual;  // fused_dual.cu (hidden width 128 / 256, two sub-tiles in flight): same pack layout
 };
 
 inline int pad64(int v) { return (v + 63) / 64 * 64; }

@@ -1,7 +1,7 @@
 """Distributions of the flow hot path: ``NormalizingFlow`` and ``DiagNormal``.
 
 Host-side mirror of zuko/distributions.py:39-138 (NormalizingFlow) and :337-363
-(DiagNormal).  Densities and inverse passes run in the B200 engine; torch provides the
+(DiagNormal).  Densities and inverse passes run in the H100 engine; torch provides the
 random numbers (``torch.randn`` on the device) and owns all memory.
 """
 

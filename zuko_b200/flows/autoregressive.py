@@ -2,7 +2,7 @@
 
 Host-side mirror of zuko/flows/autoregressive.py: ``MaskedAutoregressiveTransform``
 (:24-218) and ``MAF`` (:221-316).  Construction (orders, adjacency, masks, parameter
-initialisation) reproduces the reference bit for bit; evaluation is handed to the B200
+initialisation) reproduces the reference bit for bit; evaluation is handed to the H100
 engine as one packed ``zk_layer`` (conditioner GEMMs + fused bijector/ladj kernel).
 """
 

@@ -3,7 +3,7 @@
 Host-side mirror of zuko/lazy.py: a lazy module builds the distribution
 ``p(X | c)`` / transformation ``y = f(x | c)`` inside ``forward(c)`` so that it can be
 conditional and own parameters.  ``Flow.forward(c)`` (zuko/lazy.py:156-172) is the seam
-the B200 engine plugs in at: it returns a ``NormalizingFlow`` whose ``log_prob`` /
+the H100 engine plugs in at: it returns a ``NormalizingFlow`` whose ``log_prob`` /
 ``rsample`` are engine calls.
 """
 

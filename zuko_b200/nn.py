@@ -6,7 +6,7 @@ keys as the reference (``{2j}.weight``, ``{2j}.bias``, ``{2j}.mask``) and are in
 by the same torch initialisers in the same order, so a reference checkpoint loads
 unchanged and ``torch.manual_seed(s)`` yields bit-identical weights.
 
-``forward`` does not run torch ops: it hands the weights to the B200 engine
+``forward`` does not run torch ops: it hands the weights to the H100 engine
 (``zk_mlp_forward`` — pre-masked, packed once per parameter version).
 """
 

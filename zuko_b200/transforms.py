@@ -3,7 +3,7 @@
 Host-side mirror of the ``Transform`` protocol the reference's hot path uses
 (zuko/transforms.py): ``__call__``, ``.inv``, ``log_abs_det_jacobian(x, y)`` and Zuko's
 ``call_and_ladj(x) -> (y, ladj)`` (transforms.py:46-56).  Every method forwards to the
-C ABI of the B200 engine; no torch arithmetic runs here.
+C ABI of the H100 engine; no torch arithmetic runs here.
 
 * univariate bijectors built from explicit parameters:
   ``MonotonicRQSTransform`` (transforms.py:449-567), ``MonotonicAffineTransform``
