@@ -49,6 +49,8 @@ typedef void* zk_stream; /* cudaStream_t */
 #define ZK_UNI_RQS 2    /* MonotonicRQSTransform,    zuko/transforms.py:449-567; phi = (w[K], h[K], d[K-1]) */
 #define ZK_UNI_CRQS 3   /* CircularRQSTransform = CircularShiftTransform(bound) then RQS(bound), zuko/flows/spline.py:65-72
                            (layers only: NCSF; `bound` of the layer is pi) */
+#define ZK_UNI_GAUSS 4  /* GaussianizationTransform, zuko/transforms.py:834-875; phi = (shift[K], scale[K]), inverse by
+                           bisection on [-bound, bound] (transforms.py:609-617); element-wise layers only */
 /* base distribution of a flow */
 #define ZK_BASE_DIAG_NORMAL 0 /* DiagNormal(loc, scale)    zuko/distributions.py:337-363 */
 #define ZK_BASE_BOX_UNIFORM 1 /* BoxUniform(lower, upper)  zuko/distributions.py:366-396; base_loc = lower, base_scale = upper */
@@ -110,6 +112,15 @@ zk_status zk_affine_forward(const float* x, int64_t ldx, const float* phi, int64
 zk_status zk_affine_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld,
                             int64_t B, int D, float slope, float* x, int64_t ldx,
                             zk_stream stream);
+/* GaussianizationTransform(shift, scale, bound, eps) — transforms.py:834-875; phi = (shift[K], scale[K]) per pair.
+ * Forward: y and the closed-form ladj.  Inverse: `iterations` bisection steps on [-bound, bound] (utils.py:159-183);
+ * a y beyond the range of f returns +-(bound - half the final interval), as the reference does. */
+zk_status zk_gaussianization_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
+                                     int D, int K, float* y, int64_t ldy, float* ladj, int accumulate,
+                                     zk_stream stream);
+zk_status zk_gaussianization_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B,
+                                     int D, int K, float bound, int iterations, float* x, int64_t ldx,
+                                     zk_stream stream);
 /* SoftclipTransform(bound)                       — transforms.py:299-316 */
 zk_status zk_softclip_forward(const float* x, int64_t ldx, int64_t B, int D, float bound, float* y,
                               int64_t ldy, float* ladj, int accumulate, zk_stream stream);
@@ -184,8 +195,8 @@ typedef struct {
     int features;   /* D */
     int context;    /* C (0 = unconditional) */
     int univariate; /* ZK_UNI_* (autoregressive / coupling / elementwise) */
-    int bins;       /* K for ZK_UNI_RQS */
-    float bound;    /* spline bound B (5.0) or softclip bound */
+    int bins;       /* K for ZK_UNI_RQS, mixture components K for ZK_UNI_GAUSS */
+    float bound;    /* spline bound B (5.0), softclip bound or Gaussianization bisection bound (10.0) */
     float slope;    /* minimum slope (1e-3) */
     int passes;     /* autoregressive: number of inverse sweeps (transforms.py:994-1000) */
     const int64_t* order;         /* host (D): autoregressive order classes (MaskedAutoregressiveTransform.order,
@@ -194,6 +205,7 @@ typedef struct {
     const zk_mlp_desc* hyper;     /* conditioner; NULL for parameter-free / shared-table layers */
     const float* phi;             /* DEVICE (D, P) shared table: elementwise without context */
     const float* rotation;        /* DEVICE (D, D) R for ZK_LAYER_ROTATION */
+    int iterations;               /* ZK_UNI_GAUSS: bisection steps of the inverse, ceil(log2(2 bound / eps)) (>= 1) */
 } zk_layer_desc;
 
 zk_status zk_layer_create(const zk_layer_desc* desc, zk_layer** out);
@@ -322,6 +334,11 @@ zk_status zk_affine_backward(const float* x, int64_t ldx, const float* phi, int6
                              int D, float slope, const float* grad_y, int64_t ldgy,
                              const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi,
                              void* workspace, size_t workspace_bytes, zk_stream stream);
+/* same for GaussianizationTransform (transforms.py:834-875), P = 2K */
+zk_status zk_gaussianization_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
+                                      int D, int K, const float* grad_y, int64_t ldgy, const float* grad_ladj,
+                                      float* grad_x, int64_t ldgx, float* grad_phi, void* workspace,
+                                      size_t workspace_bytes, zk_stream stream);
 /* SoftclipTransform (transforms.py:299-316) */
 zk_status zk_softclip_backward(const float* x, int64_t ldx, int64_t B, int D, float bound,
                                const float* grad_y, int64_t ldgy, const float* grad_ladj,
@@ -396,7 +413,8 @@ zk_status zk_comm_group_end(zk_comm* comm);
 int zk_set_tc_backward(int on);
 
 /* Transcendental arithmetic of the bijector kernels: 1 (default) = MUFU rcp / ex2 / lg2
- * approximations, 0 = IEEE division + expf / logf.  Process-wide; returns the previous
+ * approximations, 0 = IEEE division + expf / logf (erf / erfc / erfcinv of the Gaussianization
+ * bijector are IEEE-library calls in both settings).  Process-wide; returns the previous
  * value.  Both settings meet the 1e-5 parity bar on the BASELINE configs (tests/). */
 int zk_set_fast_math(int on);
 /* 1 (default): an autoregressive layer whose conditioner fits the fused kernel (hidden widths

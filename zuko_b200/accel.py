@@ -47,6 +47,7 @@ _ENGINE_CALLABLES = {
     "BoxUniform": _D.BoxUniform,
     "CircularRQSTransform": _T.CircularRQSTransform,
     "CircularShiftTransform": _T.CircularShiftTransform,
+    "GaussianizationTransform": _T.GaussianizationTransform,
     "MonotonicAffineTransform": _T.MonotonicAffineTransform,
     "MonotonicRQSTransform": _T.MonotonicRQSTransform,
     "SoftclipTransform": _T.SoftclipTransform,

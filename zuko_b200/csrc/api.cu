@@ -110,6 +110,26 @@ zk_status zk_affine_inverse(const float* y, int64_t ldy, const float* phi, int64
     return launch_univariate(a, (cudaStream_t)stream);
 }
 
+zk_status zk_gaussianization_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
+                                     int D, int K, float* y, int64_t ldy, float* ladj, int accumulate,
+                                     zk_stream stream) {
+    UniArgs a;
+    a.univariate = ZK_UNI_GAUSS; a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = phi_ld; a.B = B; a.D = D;
+    a.K = K; a.bound = 10.f; a.y = y; a.ldy = ldy; a.ladj = ladj; a.accumulate = accumulate;
+    a.fast_math = g_fast_math.load() != 0;
+    return launch_univariate(a, (cudaStream_t)stream);
+}
+
+zk_status zk_gaussianization_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B,
+                                     int D, int K, float bound, int iterations, float* x, int64_t ldx,
+                                     zk_stream stream) {
+    UniArgs a;
+    a.univariate = ZK_UNI_GAUSS; a.inverse = true; a.x = y; a.ldx = ldy; a.phi = phi; a.phi_ld = phi_ld;
+    a.B = B; a.D = D; a.K = K; a.bound = bound; a.iters = iterations; a.y = x; a.ldy = ldx;
+    a.fast_math = g_fast_math.load() != 0;
+    return launch_univariate(a, (cudaStream_t)stream);
+}
+
 zk_status zk_softclip_forward(const float* x, int64_t ldx, int64_t B, int D, float bound, float* y,
                               int64_t ldy, float* ladj, int accumulate, zk_stream stream) {
     return launch_softclip(x, ldx, B, D, bound, false, y, ldy, ladj, accumulate, (cudaStream_t)stream);
@@ -303,16 +323,23 @@ static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
         l->uni = ZK_UNI_RQS;
         l->circ = true;
     }
-    l->K = d->bins; l->bound = d->bound; l->slope = d->slope; l->passes = d->passes;
+    l->K = d->bins; l->bound = d->bound; l->slope = d->slope; l->passes = d->passes; l->iters = d->iterations;
     ZK_REQUIRE(l->D >= 1, "layer_create: features=%d", l->D);
     ZK_REQUIRE(l->C >= 0, "layer_create: context=%d", l->C);
     const bool has_uni = (l->kind == ZK_LAYER_AUTOREGRESSIVE || l->kind == ZK_LAYER_COUPLING ||
                           l->kind == ZK_LAYER_ELEMENTWISE);
     if (has_uni) {
-        ZK_REQUIRE(l->uni == ZK_UNI_AFFINE || l->uni == ZK_UNI_RQS, "layer_create: univariate=%d", d->univariate);
+        ZK_REQUIRE(l->uni == ZK_UNI_AFFINE || l->uni == ZK_UNI_RQS || l->uni == ZK_UNI_GAUSS, "layer_create: univariate=%d", d->univariate);
+        if (l->uni == ZK_UNI_GAUSS) {  // the bisection inverse is element-wise only (flows/gaussianization.py:97-155)
+            if (l->kind != ZK_LAYER_ELEMENTWISE)
+                return fail(ZK_EUNSUPPORTED, "layer_create: the Gaussianization bijector is supported in element-wise layers only");
+            ZK_REQUIRE(l->K >= 1 && l->K <= 1024, "layer_create: components=%d", l->K);
+            ZK_REQUIRE(l->bound > 0.f, "layer_create: bisection bound=%g", (double)l->bound);
+            ZK_REQUIRE(l->iters >= 1 && l->iters <= 64, "layer_create: bisection iterations=%d (must be in [1, 64])", l->iters);
+        }
         if (l->uni == ZK_UNI_RQS) ZK_REQUIRE(l->K >= 1 && l->K <= 1024, "layer_create: bins=%d", l->K);
         ZK_REQUIRE(l->slope > 0.f && l->slope < 1.f, "layer_create: slope=%g", (double)l->slope);
-        l->P = (l->uni == ZK_UNI_RQS) ? 3 * l->K - 1 : 2;
+        l->P = (l->uni == ZK_UNI_RQS) ? 3 * l->K - 1 : (l->uni == ZK_UNI_GAUSS ? 2 * l->K : 2);
     }
     switch (l->kind) {
         case ZK_LAYER_AUTOREGRESSIVE: {
@@ -587,7 +614,7 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
     ZK_REQUIRE(l->C == 0 || c != nullptr, "layer needs a context of %d features", l->C);
     Arena ar(ws, ws_bytes);
     UniArgs a;
-    a.univariate = l->uni; a.inverse = true; a.B = B; a.K = l->K; a.bound = l->bound;
+    a.univariate = l->uni; a.inverse = true; a.B = B; a.K = l->K; a.bound = l->bound; a.iters = l->iters;
     a.slope = l->slope; a.fast_math = g_fast_math.load() != 0; a.circular = l->circ;
     switch (l->kind) {
         case ZK_LAYER_AUTOREGRESSIVE: {

@@ -613,7 +613,7 @@ zk_status uni_backward_entry(int uni, const float* x, int64_t ldx, const float* 
                              int64_t ldgy, const float* gl, float* gx, int64_t ldgx, float* gphi,
                              void* ws, size_t ws_bytes, cudaStream_t st) {
     ZK_REQUIRE(x && phi && B >= 0 && D > 0, "univariate backward: bad arguments");
-    const int P = (uni == ZK_UNI_RQS) ? 3 * K - 1 : 2;
+    const int P = (uni == ZK_UNI_RQS) ? 3 * K - 1 : (uni == ZK_UNI_GAUSS ? 2 * K : 2);
     UniBwdArgs u;
     u.univariate = uni; u.K = K; u.bound = bound; u.slope = slope; u.D = D;
     u.fast_math = g_fast_math.load() != 0;
@@ -663,6 +663,15 @@ zk_status zk_affine_backward(const float* x, int64_t ldx, const float* phi, int6
                              const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi,
                              void* ws, size_t ws_bytes, zk_stream stream) {
     return uni_backward_entry(ZK_UNI_AFFINE, x, ldx, phi, phi_ld, B, D, 0, 5.f, slope, grad_y, ldgy, grad_ladj,
+                              grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+zk_status zk_gaussianization_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
+                                      int D, int K, const float* grad_y, int64_t ldgy, const float* grad_ladj,
+                                      float* grad_x, int64_t ldgx, float* grad_phi, void* ws, size_t ws_bytes,
+                                      zk_stream stream) {
+    ZK_REQUIRE(K >= 1 && K <= 1024, "gaussianization backward: components must be in [1, 1024], got %d", K);
+    return uni_backward_entry(ZK_UNI_GAUSS, x, ldx, phi, phi_ld, B, D, K, 10.f, 1e-3f, grad_y, ldgy, grad_ladj,
                               grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream);
 }
 

@@ -9,6 +9,7 @@
 #include "activations.cuh"
 #include "backward.cuh"
 #include "bijector_grad.cuh"
+#include "bijector_math.cuh"
 
 namespace zk {
 
@@ -74,6 +75,10 @@ __global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const UniBwdParams
         float gxv;
         if constexpr (UNI == ZK_UNI_RQS) {
             bijgrad::rqs_backward_pair<KT, FAST>(pp, a.K, xv, gyv, glv, a.bound, a.aw, a.ad, gxv, out);
+        } else if constexpr (UNI == ZK_UNI_GAUSS) {
+            float yv, lj;
+            bij::gauss_forward_eval<KT, FAST>(pp, a.K, xv, yv, lj);
+            bijgrad::gauss_backward_pair<FAST>(pp, KT > 0 ? KT : a.K, xv, yv, gyv, glv, gxv, out);
         } else {
             bijgrad::affine_backward_pair(pp, xv, gyv, glv, a.ad, gxv, out);
         }
@@ -303,7 +308,7 @@ zk_status launch_uni_bwd_t(const UniBwdParams& p, bool fast, int grid, size_t sm
         kern<<<grid, kBwdThreads, smem, st>>>(p);
         return check_launch("uni_bwd_kernel");
     };
-    if (fast && UNI == ZK_UNI_RQS) return go(uni_bwd_kernel<UNI, KT, true>);  // affine: one expf per pair, not worth a variant
+    if (fast && UNI != ZK_UNI_AFFINE) return go(uni_bwd_kernel<UNI, KT, true>);  // affine: one expf per pair, not worth a variant
     return go(uni_bwd_kernel<UNI, KT, false>);
 }
 
@@ -313,11 +318,15 @@ zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
     ZK_REQUIRE(a.B >= 0 && a.D > 0, "univariate backward: bad shape B=%lld D=%d", (long long)a.B, a.D);
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate backward: null input");
-    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS, "univariate backward: unknown kind %d", a.univariate);
+    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS,
+               "univariate backward: unknown kind %d", a.univariate);
     int P = 2;
     if (a.univariate == ZK_UNI_RQS) {
         ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "rqs backward: bins must be in [1, 1024], got %d", a.K);
         P = 3 * a.K - 1;
+    } else if (a.univariate == ZK_UNI_GAUSS) {
+        ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "gaussianization backward: components must be in [1, 1024], got %d", a.K);
+        P = 2 * a.K;
     }
     ZK_REQUIRE(a.phi_ld == 0 || a.phi_ld >= (int64_t)a.D * P, "univariate backward: phi_ld too small");
     ZK_REQUIRE(a.slope > 0.f && a.slope < 1.f, "univariate backward: slope must be in (0, 1)");
@@ -344,6 +353,13 @@ zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
     const int64_t grid = ceil_div(a.B, R);
     ZK_REQUIRE(grid <= 0x7fffffff, "univariate backward: batch too large for one launch");
     if (a.univariate == ZK_UNI_AFFINE) return launch_uni_bwd_t<ZK_UNI_AFFINE, 0>(p, a.fast_math, (int)grid, smem, stream);
+    if (a.univariate == ZK_UNI_GAUSS) {
+        switch (a.K) {
+            case 8: return launch_uni_bwd_t<ZK_UNI_GAUSS, 8>(p, a.fast_math, (int)grid, smem, stream);
+            case 16: return launch_uni_bwd_t<ZK_UNI_GAUSS, 16>(p, a.fast_math, (int)grid, smem, stream);
+            default: return launch_uni_bwd_t<ZK_UNI_GAUSS, 0>(p, a.fast_math, (int)grid, smem, stream);
+        }
+    }
     switch (a.K) {
         case 8: return launch_uni_bwd_t<ZK_UNI_RQS, 8>(p, a.fast_math, (int)grid, smem, stream);
         case 16: return launch_uni_bwd_t<ZK_UNI_RQS, 16>(p, a.fast_math, (int)grid, smem, stream);

@@ -199,5 +199,44 @@ ZK_HD void affine_backward_pair(const float* p, float x, float gy, float gl, flo
     gp[1] = fmaf(gy * x, e, gl) * dsc(a, ad);
 }
 
+// GaussianizationTransform (transforms.py:834-875): p = (b[K] shifts, a[K] log-scales), y = f(x)
+// supplied by the caller (erfinv has no host form in the C++ library; the kernel evaluates it with
+// the forward math of bijector_math.cuh, the CPU harness reads it from the goldens).  With
+// s_k = exp(a_k), u_k = s_k x + b_k, t_k = a_k - u_k^2/2, L = logsumexp_k t_k, w_k = exp(t_k - L):
+//     dy/db_k = exp(y^2/2 + log(c/K) - u_k^2/2) =: e_k,   dy/da_k = e_k s_k x,   dy/dx = J = exp(ladj)
+//     ladj = y^2/2 + log(c/K) + L:
+//     dladj/dx = y J - sum_k w_k u_k s_k,  dladj/db_k = y e_k - w_k u_k,  dladj/da_k = y e_k s_k x + w_k (1 - u_k s_k x)
+template <bool FAST = false>
+ZK_HD void gauss_backward_pair(const float* p, int K, float x, float y, float gy, float gl, float& gx,
+                               float* gp) {
+    float mx = -INFINITY;
+    for (int k = 0; k < K; ++k) {
+        const float u = fmaf(exp_<FAST>(p[K + k]), x, p[k]);
+        mx = fmaxf(mx, fmaf(-0.5f * u, u, p[K + k]));
+    }
+    float se = 0.f;
+    for (int k = 0; k < K; ++k) {
+        const float u = fmaf(exp_<FAST>(p[K + k]), x, p[k]);
+        se += exp_<FAST>(fmaf(-0.5f * u, u, p[K + k]) - mx);
+    }
+    const float L = mx + logf(se);
+    const float h = fmaf(0.5f * y, y, logf((1.f - 1e-6f) / (float)K));  // y^2/2 + log(c/K)
+    const float G = fmaf(gl, y, gy);                                     // gy + gl y
+    float acc = 0.f;  // sum_k w_k u_k s_k
+    for (int k = 0; k < K; ++k) {
+        const float a = p[K + k];
+        const float s = exp_<FAST>(a);
+        const float u = fmaf(s, x, p[k]);
+        const float t = fmaf(-0.5f * u, u, a);
+        const float w = exp_<FAST>(t - L);
+        const float e = exp_<FAST>(h + t - a);
+        const float us = u * s;
+        acc = fmaf(w, us, acc);
+        gp[k] = fmaf(G, e, -gl * w * u);
+        gp[K + k] = fmaf(G * e * s, x, gl * w * fmaf(-us, x, 1.f));
+    }
+    gx = fmaf(G, exp_<FAST>(h + L), -gl * acc);
+}
+
 }  // namespace bijgrad
 }  // namespace zk

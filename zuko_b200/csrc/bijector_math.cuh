@@ -206,6 +206,104 @@ __device__ __forceinline__ float rqs_inverse_eval(const Bin& b, float y) {
     return b.inside ? x : y;
 }
 
+// ---------------------------------------------------------------------------
+// Gaussianization: f(x) = sqrt2 erfinv(c/K sum_k erf(u_k / sqrt2)), u_k = exp(a_k) x + b_k,
+// c = 1 - 1e-6 (GaussianizationTransform.f, transforms.py:867-873).  p points at the pair's
+// P = 2K raw parameters: p[0..K) shifts b, p[K..2K) unconstrained log-scales a.
+//
+// The mixture CDF is carried as its two tails, never as erf sums near +-1:
+//   tp = 1 - c/K sum erf(v_k) = 1e-6 + c/K sum erfc(v_k)     (upper tail, = P[Y > y])
+//   tn = 1 + c/K sum erf(v_k) = 1e-6 + c/K sum erfc(-v_k)    (lower tail), tp + tn = 2
+// One erfcf(|v_k|) per component gives both sums without cancellation: the small term goes
+// to the tail it belongs to, 2 - it to the other.  erf / erfc have no MUFU form: FAST only
+// changes the exp / log around them.
+// ---------------------------------------------------------------------------
+constexpr float kRsqrt2 = 0.7071067811865476f;
+constexpr float kSqrt2 = 1.4142135623730951f;
+constexpr float kGaussFloor = 1e-6f;  // 1 - c
+
+// tail sums of the K components at x; sp / sn = sum erfc(v_k) / sum erfc(-v_k)
+template <int KT, bool FAST>
+__device__ __forceinline__ void gauss_tails(const float* __restrict__ p, int Krt, const float* sreg,
+                                            float x, float& sp, float& sn) {
+    const int K = KT > 0 ? KT : Krt;
+    sp = 0.f;
+    sn = 0.f;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        const float s = KT > 0 ? sreg[k] : zexp<FAST>(p[K + k]);
+        const float v = fmaf(s, x, p[k]) * kRsqrt2;
+        const float e = erfcf(fabsf(v));
+        const bool pos = v >= 0.f;
+        sp += pos ? e : 2.f - e;
+        sn += pos ? 2.f - e : e;
+    }
+}
+
+// y = f(x) from the two tail sums (cK = c / K)
+__device__ __forceinline__ float gauss_from_tails(float sp, float sn, float cK) {
+    return sp <= sn ? kSqrt2 * erfcinvf(fmaf(cK, sp, kGaussFloor))
+                    : -kSqrt2 * erfcinvf(fmaf(cK, sn, kGaussFloor));
+}
+
+// forward value and closed-form log-derivative
+//   ladj = y^2/2 + log(c/K) + logsumexp_k(a_k - u_k^2/2)
+template <int KT, bool FAST>
+__device__ __forceinline__ void gauss_forward_eval(const float* __restrict__ p, int Krt, float x,
+                                                   float& y, float& ladj) {
+    const int K = KT > 0 ? KT : Krt;
+    const float cK = (1.f - kGaussFloor) / (float)K;
+    float sp = 0.f, sn = 0.f;
+    float mx = -INFINITY, se = 0.f;  // online logsumexp
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        const float a = p[K + k];
+        const float u = fmaf(zexp<FAST>(a), x, p[k]);
+        const float v = u * kRsqrt2;
+        const float e = erfcf(fabsf(v));
+        const bool pos = v >= 0.f;
+        sp += pos ? e : 2.f - e;
+        sn += pos ? 2.f - e : e;
+        const float t = fmaf(-0.5f * u, u, a);
+        if (t > mx) {
+            se = fmaf(se, zexp<FAST>(mx - t), 1.f);
+            mx = t;
+        } else {
+            se += zexp<FAST>(t - mx);
+        }
+    }
+    y = gauss_from_tails(sp, sn, cK);
+    ladj = fmaf(0.5f * y, y, zlog<FAST>(cK) + mx + zlog<FAST>(se));
+}
+
+// inverse: the reference's bisection (utils.py:159-183) on [-bound, bound], `iters` halvings,
+// x = midpoint of the final interval.  "f(m) < y" is decided on the tail of y's sign:
+// y >= 0: tp(m) > erfc(y / sqrt2);  y < 0: tn(m) < erfc(-y / sqrt2).
+template <int KT, bool FAST>
+__device__ __forceinline__ float gauss_inverse_eval(const float* __restrict__ p, int Krt, float y,
+                                                    float bound, int iters) {
+    const int K = KT > 0 ? KT : Krt;
+    constexpr int KA = KT > 0 ? KT : 1;
+    float sreg[KA];
+    if constexpr (KT > 0) {
+#pragma unroll
+        for (int k = 0; k < KT; ++k) sreg[k] = zexp<FAST>(p[K + k]);
+    }
+    const float cK = (1.f - kGaussFloor) / (float)K;
+    const bool upper = y >= 0.f;
+    const float target = erfcf(fabsf(y) * kRsqrt2);
+    float lo = -bound, hi = bound;
+    for (int it = 0; it < iters; ++it) {
+        const float m = 0.5f * (lo + hi);
+        float sp, sn;
+        gauss_tails<KT, FAST>(p, K, sreg, m, sp, sn);
+        const bool below = upper ? (fmaf(cK, sp, kGaussFloor) > target) : (fmaf(cK, sn, kGaussFloor) < target);
+        lo = below ? m : lo;
+        hi = below ? hi : m;
+    }
+    return 0.5f * (lo + hi);
+}
+
 
 }  // namespace bij
 }  // namespace zk

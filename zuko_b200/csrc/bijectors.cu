@@ -4,7 +4,10 @@
 //   phi (B, D, P):  x, phi  ->  y, sum_d log|dy/dx|  (+ optional DiagNormal log-prob)
 // replacing the ~95 eager aten ops of MonotonicRQSTransform.__init__ +
 // call_and_ladj + DependentTransform (zuko/transforms.py:469-490, 554-567, 210-214)
-// and the ~10 of MonotonicAffineTransform (zuko/transforms.py:426-446).
+// and the ~10 of MonotonicAffineTransform (zuko/transforms.py:426-446), and
+// GaussianizationTransform (zuko/transforms.py:834-875): K erfc terms and the closed-form
+// ladj instead of the reference's autograd call per forward (transforms.py:623-637), and its
+// bisection inverse (transforms.py:609-617, utils.py:159-183) run in registers.
 //
 // Data movement: a CTA owns a tile of R consecutive sample rows.  Their phi block is
 // one contiguous range of R*D*P floats in HBM; it is staged into shared memory with a
@@ -45,6 +48,7 @@ struct UniParams {
     int rows_per_tile;
     int circ;      // RQS: circular shift by `bound` before the spline (forward) / after it (inverse)
     int use_bulk;  // host-side verdict: alignment rules for cp.async.bulk hold for full tiles
+    int iters;     // Gaussianization inverse: bisection steps
 };
 
 // UNI: ZK_UNI_*; KT: compile-time bins (0 = runtime K); INVERSE; FAST math
@@ -105,6 +109,12 @@ __global__ void __launch_bounds__(kUniThreads) uni_kernel(const UniParams a) {
                     Bin b = rqs_select<KT, FAST, true>(pp, a.K, xv, a.bound, a.aw, a.ad);
                     yv = rqs_inverse_eval<FAST>(b, xv);
                     if (a.circ) yv = circ_shift(yv, a.bound);
+                }
+            } else if constexpr (UNI == ZK_UNI_GAUSS) {
+                if constexpr (!INVERSE) {
+                    gauss_forward_eval<KT, FAST>(pp, a.K, xv, yv, lj);
+                } else {
+                    yv = gauss_inverse_eval<KT, FAST>(pp, a.K, xv, a.bound, a.iters);
                 }
             } else {  // affine, transforms.py:435-446: phi = (shift, unconstrained log-scale)
                 const float shift = pp[0];
@@ -169,6 +179,13 @@ template <bool INVERSE>
 zk_status launch_uni_dir(const UniParams& p, int uni, bool fast, int grid, size_t smem,
                          cudaStream_t st) {
     if (uni == ZK_UNI_AFFINE) return launch_uni_t<ZK_UNI_AFFINE, 0, INVERSE>(p, fast, grid, smem, st);
+    if (uni == ZK_UNI_GAUSS) {
+        switch (p.K) {
+            case 8: return launch_uni_t<ZK_UNI_GAUSS, 8, INVERSE>(p, fast, grid, smem, st);
+            case 16: return launch_uni_t<ZK_UNI_GAUSS, 16, INVERSE>(p, fast, grid, smem, st);
+            default: return launch_uni_t<ZK_UNI_GAUSS, 0, INVERSE>(p, fast, grid, smem, st);
+        }
+    }
     switch (p.K) {
         case 4: return launch_uni_t<ZK_UNI_RQS, 4, INVERSE>(p, fast, grid, smem, st);
         case 8: return launch_uni_t<ZK_UNI_RQS, 8, INVERSE>(p, fast, grid, smem, st);
@@ -183,12 +200,17 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     ZK_REQUIRE(a.B >= 0 && a.D > 0, "univariate: bad shape B=%lld D=%d", (long long)a.B, a.D);
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate: null input");
-    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS,
+    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS,
                "univariate: unknown kind %d", a.univariate);
     int P = 2;
     if (a.univariate == ZK_UNI_RQS) {
         ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "rqs: bins must be in [1, 1024], got %d", a.K);
         P = 3 * a.K - 1;
+    } else if (a.univariate == ZK_UNI_GAUSS) {
+        ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "gaussianization: components must be in [1, 1024], got %d", a.K);
+        ZK_REQUIRE(a.bound > 0.f, "gaussianization: bound must be positive");
+        if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "gaussianization: bisection steps must be in [1, 64], got %d", a.iters);
+        P = 2 * a.K;
     }
     ZK_REQUIRE(a.phi_ld == 0 || a.phi_ld >= (int64_t)a.D * P, "univariate: phi_ld too small");
     ZK_REQUIRE(a.slope > 0.f && a.slope < 1.f, "univariate: slope must be in (0, 1)");
@@ -201,6 +223,7 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     p.log_prob = a.log_prob; p.base_loc = a.base_loc; p.base_scale = a.base_scale;
     p.dim_map = a.dim_map; p.B = a.B; p.D = a.D; p.K = a.K; p.P = P; p.bound = a.bound;
     p.circ = (a.circular && a.univariate == ZK_UNI_RQS) ? 1 : 0;
+    p.iters = a.iters;
     const float absL = fabsf(logf(a.slope));
     p.aw = 2.f / absL;
     p.ad = 1.f / absL;

@@ -3,10 +3,12 @@
 from .autoregressive import MAF, MaskedAutoregressiveTransform
 from .coupling import NICE, GeneralCouplingTransform, RealNVP
 from .elementwise import ElementWiseTransform
+from .gaussianization import GF
 from .spline import NCSF, NSF
 from ..lazy import Flow, UnconditionalDistribution, UnconditionalTransform
 
 __all__ = [
+    "GF",
     "MAF",
     "NCSF",
     "NICE",

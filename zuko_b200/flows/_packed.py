@@ -14,7 +14,13 @@ from torch import Size
 from .. import _engine as E
 import math
 
-from ..transforms import CircularRQSTransform, MonotonicAffineTransform, MonotonicRQSTransform
+from ..transforms import (
+    CircularRQSTransform,
+    GaussianizationTransform,
+    MonotonicAffineTransform,
+    MonotonicRQSTransform,
+    bisection_steps,
+)
 
 
 def resolve_univariate(univariate: Callable, shapes: Sequence[Size]) -> dict:
@@ -53,10 +59,26 @@ def resolve_univariate(univariate: Callable, shapes: Sequence[Size]) -> dict:
             raise NotImplementedError(f"zuko_b200: unsupported CircularRQSTransform arguments {sorted(extra)}")
         K = shapes[0][0]
         return dict(kind=E.ZK_UNI_CRQS, bins=K, bound=math.pi, slope=float(kwargs.get("slope", 1e-3)), total=3 * K - 1)
+    if f is GaussianizationTransform:
+        if len(shapes) != 2 or shapes[0] != shapes[1] or len(shapes[0]) != 1:
+            raise ValueError(f"GaussianizationTransform expects shapes [(K,), (K,)], got {shapes}")
+        extra = set(kwargs) - {"bound", "eps"}
+        if extra:
+            raise NotImplementedError(f"zuko_b200: unsupported GaussianizationTransform arguments {sorted(extra)}")
+        K = shapes[0][0]
+        bound, eps = float(kwargs.get("bound", 10.0)), float(kwargs.get("eps", 1e-6))
+        return dict(kind=E.ZK_UNI_GAUSS, bins=K, bound=bound, slope=1e-3, total=2 * K, iterations=bisection_steps(bound, eps))
     raise NotImplementedError(
         f"zuko_b200: univariate transformation {getattr(f, '__name__', f)!r} is not implemented by the engine "
-        "(supported: MonotonicAffineTransform, MonotonicRQSTransform, CircularRQSTransform)"
+        "(supported: MonotonicAffineTransform, MonotonicRQSTransform, CircularRQSTransform, GaussianizationTransform)"
     )
+
+
+def refuse_elementwise_only(uni: dict, layer: str) -> None:
+    """The Gaussianization bijector's bisection inverse runs per element: the engine takes it in
+    element-wise layers only (flows/gaussianization.py:97-155)."""
+    if uni["kind"] == E.ZK_UNI_GAUSS:
+        raise NotImplementedError(f"zuko_b200: GaussianizationTransform is supported in element-wise layers only, not in {layer}")
 
 
 class OwnedLayer:
@@ -193,9 +215,12 @@ class PackedLayerMixin:
     def _base_desc(self, kind: int) -> E.LayerDesc:
         u = self._uni
         return E.LayerDesc(kind=kind, features=self.features, context=self.context, univariate=u["kind"],
-                           bins=u["bins"], bound=u["bound"], slope=u["slope"], passes=getattr(self, "passes", 0))  # fmt: skip
+                           bins=u["bins"], bound=u["bound"], slope=u["slope"], passes=getattr(self, "passes", 0),
+                           iterations=u.get("iterations", 0))  # fmt: skip
 
     def _describe_base(self) -> str:
+        if self._uni["kind"] == E.ZK_UNI_GAUSS:
+            return "GaussianizationTransform(components=%d)" % self._uni["bins"]
         if self._uni["kind"] == E.ZK_UNI_CRQS:
             return "CircularRQSTransform(bins=%d)" % self._uni["bins"]
         return "MonotonicRQSTransform(bins=%d)" % self._uni["bins"] if self._uni["kind"] == E.ZK_UNI_RQS else "MonotonicAffineTransform()"

@@ -24,7 +24,7 @@ from ..distributions import DiagNormal
 from ..lazy import Flow, LazyTransform, UnconditionalDistribution
 from ..nn import MaskedMLP
 from ..transforms import AutoregressiveTransform, MonotonicAffineTransform
-from ._packed import PackedLayerMixin, resolve_univariate, total_of
+from ._packed import PackedLayerMixin, refuse_elementwise_only, resolve_univariate, total_of
 from .elementwise import ElementWiseTransform
 
 
@@ -111,6 +111,7 @@ class MaskedAutoregressiveTransform(PackedLayerMixin, LazyTransform):
         self.univariate, self.shapes = univariate, shapes
         self.total = total_of(shapes)
         self._uni = resolve_univariate(univariate, shapes)
+        refuse_elementwise_only(self._uni, "MaskedAutoregressiveTransform")
         self.features, self.context = features, context
         self.register_buffer("order", None)
 

@@ -7,7 +7,7 @@ C ABI of the H100 engine; no torch arithmetic runs here.
 
 * univariate bijectors built from explicit parameters:
   ``MonotonicRQSTransform`` (transforms.py:449-567), ``MonotonicAffineTransform``
-  (:412-446), ``SoftclipTransform`` (:286-316);
+  (:412-446), ``GaussianizationTransform`` (:834-875), ``SoftclipTransform`` (:286-316);
 * linear maps: ``PermutationTransform`` (:1182-1214), ``RotationTransform`` (:1217-1244);
 * packed conditional layers produced by the lazy modules in ``zuko_b200.flows``:
   ``AutoregressiveTransform`` (:966-1007), ``CouplingTransform`` (:1010-1073),
@@ -25,6 +25,7 @@ __all__ = [
     "ComposedTransform",
     "CouplingTransform",
     "DependentTransform",
+    "GaussianizationTransform",
     "MonotonicAffineTransform",
     "MonotonicRQSTransform",
     "PermutationTransform",
@@ -150,6 +151,8 @@ def _uni_forward(kind: int, K: int, bound: float, slope: float, x2: Tensor, phi:
     with torch.cuda.device(x2.device):
         if kind == E.ZK_UNI_RQS:
             E.check(L.zk_rqs_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, K, bound, slope, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
+        elif kind == E.ZK_UNI_GAUSS:
+            E.check(L.zk_gaussianization_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, K, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
         elif kind == E.ZK_UNI_AFFINE:
             E.check(L.zk_affine_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, slope, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
         else:
@@ -159,8 +162,8 @@ def _uni_forward(kind: int, K: int, bound: float, slope: float, x2: Tensor, phi:
 
 class _UniFunction(torch.autograd.Function):
     """Autograd seam of the explicit-parameter bijectors: backward = ``zk_rqs_backward`` /
-    ``zk_affine_backward`` / ``zk_softclip_backward`` (reverse mode of transforms.py:469-567,
-    426-446, 299-316)."""
+    ``zk_affine_backward`` / ``zk_gaussianization_backward`` / ``zk_softclip_backward`` (reverse mode
+    of transforms.py:469-567, 426-446, 834-875, 299-316)."""
 
     @staticmethod
     def forward(ctx, kind, K, bound, slope, ld, x2, phi):  # noqa: ANN001
@@ -196,6 +199,8 @@ class _UniFunction(torch.autograd.Function):
                     0 if ws is None else ws.numel(), st)  # fmt: skip
             if kind == E.ZK_UNI_RQS:
                 E.check(L.zk_rqs_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, K, bound, slope, *args))
+            elif kind == E.ZK_UNI_GAUSS:
+                E.check(L.zk_gaussianization_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, K, *args))
             else:
                 E.check(L.zk_affine_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, slope, *args))
         return None, None, None, None, None, gx, gphi
@@ -283,6 +288,46 @@ class MonotonicAffineTransform(EngineTransform):
         with torch.cuda.device(y2.device):
             E.check(E.lib().zk_affine_inverse(y2.data_ptr(), 1, phi.data_ptr(), ld, y2.shape[0], 1, self.slope,
                                               x.data_ptr(), 1, E.stream_ptr(y2.device)))  # fmt: skip
+        return x.reshape(shape)
+
+
+def bisection_steps(bound: float, eps: float) -> int:
+    """Iterations of the reference's bisection inverse on ``[-bound, bound]`` (transforms.py:609-617)."""
+    return math.ceil(math.log2(2 * bound / eps))
+
+
+class GaussianizationTransform(EngineTransform):
+    """``f(x) = Phi^-1(c/K sum_k Phi(exp(a_k) x + b_k))``, ``c = 1 - 1e-6``, with ``shift`` b and unconstrained
+    ``scale`` a of shape ``(*, K)`` (zuko/transforms.py:834-875).  ``zk_gaussianization_forward`` evaluates y and the
+    closed-form ladj; the inverse runs the reference's ``ceil(log2(2 bound / eps))`` bisection steps on
+    ``[-bound, bound]`` (transforms.py:609-617) in ``zk_gaussianization_inverse``."""
+
+    domain = constraints.real
+    codomain = constraints.real
+
+    def __init__(self, shift: Tensor, scale: Tensor, bound: float = 10.0, eps: float = 1e-6) -> None:
+        super().__init__()
+        shift, scale = torch.broadcast_tensors(shift, scale)
+        self.phi = torch.cat((shift, scale), dim=-1)  # (*, 2K): layout of flows/gaussianization.py:91-92
+        self.components = shift.shape[-1]
+        self.bound, self.eps = float(bound), float(eps)
+        self.iterations = bisection_steps(self.bound, self.eps)
+
+    def __repr__(self) -> str:
+        return f"{type(self).__name__}(components={self.components})"
+
+    def call_and_ladj(self, x: Tensor) -> tuple[Tensor, Tensor]:
+        x2, phi, ld, shape = _elementwise(self.phi, x, 2 * self.components)
+        y, ladj = _uni_call(E.ZK_UNI_GAUSS, self.components, self.bound, 1e-3, x2, phi, ld)
+        return y.reshape(shape), ladj.reshape(shape)
+
+    def _inverse(self, y: Tensor) -> Tensor:
+        _no_grad_inverse(y, self.phi)
+        y2, phi, ld, shape = _elementwise(self.phi.detach(), y.detach(), 2 * self.components)
+        x = torch.empty_like(y2)
+        with torch.cuda.device(y2.device):
+            E.check(E.lib().zk_gaussianization_inverse(y2.data_ptr(), 1, phi.data_ptr(), ld, y2.shape[0], 1, self.components,
+                                                       self.bound, self.iterations, x.data_ptr(), 1, E.stream_ptr(y2.device)))  # fmt: skip
         return x.reshape(shape)
 
 
