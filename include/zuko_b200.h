@@ -229,6 +229,9 @@ size_t zk_layer_workspace_bytes(const zk_layer* layer, int64_t B);
  * out[1] = non-zero 64 x 64 weight tiles per row tile, out[2] = MACs ISSUED per sample row (non-zero tiles only, all
  * split-bf16 terms), out[3] = dense MACs per sample row (what nn.py:218 executes). */
 int zk_layer_fused_info(const zk_layer* layer, double* out);
+/* Rows per tile of the fused layer kernel for this layer, chosen from its shape: 128 (two consumer warpgroups
+ * share every streamed weight tile), 64, or 0 when the layer does not run as the fused kernel.  Read-only. */
+int zk_layer_fused_tile_rows(const zk_layer* layer);
 /* 1 when the layer's inverse runs as the dimension-sequential kernel (one launch, emits the ladj): the
  * precondition for using it as an inverted member of a zk_flow_desc. */
 int zk_layer_sequential_inverse(const zk_layer* layer);

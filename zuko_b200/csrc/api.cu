@@ -475,6 +475,11 @@ int zk_layer_fused_info(const zk_layer* l, double* out) {
     return kind;
 }
 
+int zk_layer_fused_tile_rows(const zk_layer* l) {
+    if (!l || l->kind != ZK_LAYER_AUTOREGRESSIVE || !l->hyper || l->circ) return 0;
+    return fused_tile_rows(l->hyper, l->uni, l->K, l->D, l->C);
+}
+
 size_t zk_layer_workspace_bytes(const zk_layer* l, int64_t B) {
     if (!l || B <= 0) return 0;
     switch (l->kind) {
@@ -1044,8 +1049,8 @@ zk_status get_pipe(HostPipe** out) {
 }  // extern "C"
 
 /* Row chunks of the host pipeline.  The H2D copies run ahead of the compute, so a call costs copy(first chunk) + compute(all) +
-   a per-launch ramp per chunk: the first chunk is ONE wave of the persistent kernels (a wave = one 64-row tile of the
-   fused layer kernel per SM; chunks are whole waves, a 3.46-wave chunk runs as 4), the later ones grow by <= 1.7x — with two
+   a per-launch ramp per chunk: the first chunk is ONE wave of the persistent kernels (a wave = one row tile of the
+   fused layer kernel per SM, host_wave; chunks are whole waves, a 3.46-wave chunk runs as 4), the later ones grow by <= 1.7x — with two
    staging slots the copy of chunk k starts when chunk k-2 is done and has to finish within the compute of
    chunk k-1 — up to `max_chunk` (what the workspace holds).  Small batches: eight equal chunks as before. */
 std::vector<int64_t> host_chunk_plan(int64_t B, int64_t wave, int64_t max_chunk) {
@@ -1069,6 +1074,13 @@ std::vector<int64_t> host_chunk_plan(int64_t B, int64_t wave, int64_t max_chunk)
     return plan;
 }
 
+// rows of one wave: a row tile of the fused layer kernel per SM, at the tallest tile the flow's layers run with
+static int64_t host_wave(const zk_flow_desc* f) {
+    int rows = 64;
+    for (int i = 0; f->layers && i < f->n_layers; ++i) rows = std::max(rows, zk_layer_fused_tile_rows(f->layers[i]));
+    return (int64_t)sm_count() * rows;
+}
+
 static size_t host_pipe_need(const zk_flow_desc* f, int64_t n) {
     const size_t D = (size_t)f->features, C = (size_t)f->context;
     return 2 * (a256((size_t)n * D * 4) + a256((size_t)n * C * 4) + a256((size_t)n * 4)) + a256(C * 4) +
@@ -1079,7 +1091,7 @@ extern "C" {
 
 size_t zk_flow_host_workspace_bytes(const zk_flow_desc* f, int64_t B) {
     if (!f || B <= 0) return 1024;
-    const int64_t wave = (int64_t)sm_count() * 64;
+    const int64_t wave = host_wave(f);
     int64_t big = 0;
     for (int64_t n : host_chunk_plan(B, wave, B)) big = std::max(big, n);
     return host_pipe_need(f, big) + 4096;
@@ -1111,7 +1123,7 @@ zk_status zk_flow_log_prob_host(const zk_flow_desc* f, const float* xh, int64_t 
     const size_t stage_row = (size_t)(D + (bc ? 0 : C) + 1) * 4;
     // chunk plan (host_chunk_plan): the step's time is the FIRST chunk's copy plus the compute of all of them,
     // so the first chunk is one wave and the later ones grow; bounded by the workspace
-    const int64_t wave = (int64_t)sm_count() * 64;
+    const int64_t wave = host_wave(f);
     auto need = [&](int64_t n) { return host_pipe_need(f, n); };
     int64_t Bmax = B;
     while (Bmax > 1 && need(Bmax) > ws_bytes) Bmax = (Bmax > wave) ? std::max<int64_t>(wave, (Bmax / 2 / wave) * wave) : (Bmax + 1) / 2;

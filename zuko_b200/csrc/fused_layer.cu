@@ -1,12 +1,11 @@
 // zuko_b200 — ONE kernel per flow layer: conditioner (all linear layers) + bijector + ladj.
 //
-//   x, c  --(bf16 hi/lo split, in-kernel)-->  A operand in SHARED MEMORY (64 rows x up to 512 columns)
+//   x, c  --(bf16 hi/lo split, in-kernel)-->  A operand in SHARED MEMORY (64 or 128 rows x up to 512 columns)
 //   for every linear layer:  wgmma  D[registers] += A[smem] * W[smem]^T
 //        W is streamed from L2 by TMA as 64 x 64 tiles (hi + lo planes) through a ring of mbarrier
 //        slots; the all-zero tiles of the degree-sorted masked matrices are never loaded or multiplied;
-//        hidden layers : the two consumer warpgroups split the layer's 64-column chunks (chunk ch
-//                        belongs to warpgroup ch % 2, at most four 64 x 64 fp32 accumulators each),
-//                        and once BOTH have finished reading A they overwrite it in place with the
+//        hidden layers : at most four 64 x 64 fp32 accumulators per consumer warpgroup; once every
+//                        reader of an A operand is done with it, it is overwritten in place with the
 //                        layer's output (bias, activation, bf16 hi/lo split): activations never
 //                        leave shared memory;
 //        last layer    : its rows are regrouped so that a 64-row chunk holds whole dims; the
@@ -20,11 +19,19 @@
 // 554-567 (RQS) or 426-446 (affine), transforms.py:210-214 (sum over D), and on the last
 // layer of a flow distributions.py:115-119 + torch normal.py:87-102 (DiagNormal log-prob).
 //
-// Warp roles (384 threads, 1 CTA / SM, persistent over 64-row tiles):
-//   warpgroup 0     W producer (one thread: TMA loads in a fixed tile order, each tile into the ring of
-//                   the warpgroup that multiplies it — a ring has ONE consumer that takes every slot in
-//                   order, so its mbarrier phases can never be lapped)
+// Warp roles (384 threads, 1 CTA / SM, persistent over row tiles).  The row tile is 64 or 128 rows,
+// chosen by the launcher from the shape (fused_plan):
+//   warpgroup 0     W producer (one thread: TMA loads in a fixed tile order)
 //   warpgroups 1-2  consumers: input staging, MMAs, epilogues
+// 64-row tiles: the consumers split the layers' 64-column chunks (chunk ch belongs to warpgroup ch % 2); each
+//   tile goes into the ring of the warpgroup that multiplies it — a ring has ONE consumer that takes every
+//   slot in order, so its mbarrier phases can never be lapped.
+// 128-row tiles: warpgroup 1 owns rows 0-63 of the tile and warpgroup 2 rows 64-127, each with its own A
+//   operand; both multiply EVERY weight tile (one ring, two arrivals per slot, neither consumer skips a
+//   slot), so a tile brought in by TMA feeds 128 rows.  Hidden-layer MMAs are asynchronous (one group per tile,
+//   the next tile issued before waiting, a slot released one tile late); an output chunk's tiles are issued as
+//   one asynchronous batch that completes before its bijector runs.  The warpgroups only meet at the W ring.
+//   The producer runs on 40 registers and the consumers on 232 (setmaxnreg).
 
 #include <string.h>
 
@@ -42,17 +49,18 @@ namespace {
 
 using namespace bij;
 
-constexpr int FM = 64;              // rows per tile (one wgmma M)
+constexpr int FM = 64;              // rows per wgmma M (and per consumer warpgroup)
 constexpr int FK = 64;              // bf16 per K block (128-byte swizzle row) = columns per chunk
 constexpr int F_MAXKB = 8;          // A operand: up to 8 K blocks = 512 columns
-constexpr int F_MAX_STAGES = 8;     // the W ring is as deep as shared memory allows (see launch_fused_layer)
+constexpr int F_MAX_STAGES = 8;     // the W ring is as deep as shared memory allows (see fused_plan)
+constexpr int F_WIDE_MAXKB = 4;     // 128-row tiles: four accumulators per consumer hold every hidden chunk
 constexpr int F_THREADS = 384;
 constexpr uint32_t F_TILE = FM * FK * 2;  // 8 KB: one plane of a 64 x 64 tile
 constexpr uint32_t F_STAGE = 2 * F_TILE;  // hi + lo
-constexpr int F_SROW = 65;                // floats per row of the output-layer staging buffer (odd: no bank conflicts)
-constexpr uint32_t F_STAGING_BYTES = 2u * FM * F_SROW * 4u;          // one buffer per consumer warpgroup
-constexpr uint32_t F_AUX_BYTES = 4u * FM * 4u + 2u * F_MAX_STAGES * 8u;  // ladj partials [4][64] + barriers
 constexpr uint32_t F_SMEM_MAX = 232448;   // 227 KB per block on sm_90
+
+// floats per row of the output-layer staging buffer: the chunk's DPC * P parameters, made odd (no bank conflicts)
+__host__ __device__ constexpr int f_srow(int dpc_p) { return dpc_p | 1; }
 
 struct FusedParams {
     CUtensorMap mapW[ZK_FUSED_MAX_LINEAR];
@@ -67,7 +75,7 @@ struct FusedParams {
     int n_terms;        // 3 (split bf16) or 1
     int act;            // hidden activation: 1 ReLU, else ZK_ACT_* (GACT instantiation)
     int M;
-    int n_stages;       // slots of the W rings (16 KB each), half per consumer warpgroup
+    int n_stages;       // slots of the W ring(s), 16 KB each (64-row tiles: half per consumer warpgroup)
     const float* x; int64_t ldx;
     const float* c; int64_t ldc;
     float* y; int64_t ldy;
@@ -91,32 +99,39 @@ __device__ __forceinline__ void tile_mma(float (&acc)[4][32], int q, uint32_t a_
     for (int i = 0; i < 4; ++i) acc_fence(acc[i]);
 }
 
-template <int UNI, int KT, bool FAST, bool GACT>
+// NT: split-bf16 terms as a compile-time constant (128-row tiles: no branch between the asynchronous MMAs of an
+// accumulator), or 0 to read p.n_terms
+template <int UNI, int KT, bool FAST, bool GACT, int ROWS, int NT>
 __global__ void __launch_bounds__(F_THREADS, 1)
 fused_layer_kernel(const __grid_constant__ FusedParams p) {
     using Cfg = LastCfg<UNI, KT>;
     constexpr int P = Cfg::P, DPC = Cfg::DPC;
-    static_assert(DPC * P <= FK, "a last-layer chunk must fit 64 columns");
+    constexpr int NP = DPC * P, SROW = f_srow(NP);  // staged columns of an output chunk, staging row stride
+    constexpr bool WIDE = (ROWS == 128);
+    static_assert(NP <= FK, "a last-layer chunk must fit 64 columns");
+    static_assert(ROWS == 64 || ROWS == 128, "row tile: one or two wgmma M");
+    const int n_terms = NT ? NT : p.n_terms;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    // [W ring: n_stages x 16 KB][A: 2 planes x KBA x 8 KB][staging 2 x 64 x 65 fp32][ladj partials][barriers]
+    // [W ring: n_stages x 16 KB][A: ROWS / 64 x 2 planes x KBA x 8 KB][staging 2 x 64 x SROW fp32]
+    // [ladj partials 4 x ROWS][barriers]
     const int NS = p.n_stages;
     uint8_t* sW = smem;
     uint8_t* sA = smem + (size_t)NS * F_STAGE;
     const uint32_t a_plane = (uint32_t)p.KBA * F_TILE;
-    float* s_stage = (float*)(sA + 2 * (size_t)a_plane);
-    float* s_part = s_stage + 2 * FM * F_SROW;               // [4][64]
-    uint64_t* full = (uint64_t*)(s_part + 4 * FM);           // [F_MAX_STAGES] TMA -> consumer
+    float* s_stage = (float*)(sA + (ROWS / FM) * 2 * (size_t)a_plane);
+    float* s_part = s_stage + 2 * FM * SROW;
+    uint64_t* full = (uint64_t*)(s_part + 4 * ROWS);         // [F_MAX_STAGES] TMA -> consumer
     uint64_t* empty = full + F_MAX_STAGES;                   // [F_MAX_STAGES] consumer -> TMA
-    const int NR = NS / 2;                                   // ring of warpgroup g: slots [g NR, g NR + NR)
+    const int NR = WIDE ? NS : NS / 2;                       // slots per ring (64 rows: ring g = [g NR, g NR + NR))
 
     const int L = p.n_linear;
-    const int m_tiles = (p.M + FM - 1) / FM;
+    const int m_tiles = (p.M + ROWS - 1) / ROWS;
     const int nch = p.H / FK;  // hidden chunks = K blocks of every layer after the first
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+        for (int s = 0; s < NS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], WIDE ? 2 : 1); }
         fence_mbar_init();
     }
     __syncthreads();
@@ -126,17 +141,18 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
         // ======================= W producer =======================
         // tile order (the consumers walk the same one): hidden layers K block by K block, each over
         // its chunks; the output layer chunk by chunk, each over its K blocks
+        if constexpr (WIDE) setmaxnreg_dec<40>();
         if (threadIdx.x == 0) {
-            const uint32_t bytes = (p.n_terms == 3) ? F_STAGE : F_TILE;
+            const uint32_t bytes = (n_terms == 3) ? F_STAGE : F_TILE;
             int rs[2] = {0, 0};
             uint32_t rph[2] = {0u, 0u};
-            auto load = [&](int l, int ch, int kb) {  // chunk ch is multiplied by consumer warpgroup ch % 2
-                const int o = ch & 1, s = o * NR + rs[o];
+            auto load = [&](int l, int ch, int kb) {  // 64 rows: chunk ch is multiplied by consumer warpgroup ch % 2
+                const int o = WIDE ? 0 : (ch & 1), s = o * NR + rs[o];
                 mbar_wait(&empty[s], rph[o] ^ 1);
                 uint8_t* dst = sW + (size_t)s * F_STAGE;
                 mbar_arrive_expect_tx(&full[s], bytes);
                 tma_load_3d(dst, &p.mapW[l], &full[s], kb * FK, ch * FK, 0);
-                if (p.n_terms == 3) tma_load_3d(dst + F_TILE, &p.mapW[l], &full[s], kb * FK, ch * FK, 1);
+                if (n_terms == 3) tma_load_3d(dst + F_TILE, &p.mapW[l], &full[s], kb * FK, ch * FK, 1);
                 if (++rs[o] == NR) { rs[o] = 0; rph[o] ^= 1; }
             };
             for (int t = blockIdx.x; t < m_tiles; t += gridDim.x) {
@@ -155,25 +171,32 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
     }
 
     // ======================= consumers =======================
-    const int cw = wg - 1;                       // chunk parity this warpgroup owns
+    if constexpr (WIDE) setmaxnreg_inc<232>();
+    const int cw = wg - 1;  // 64 rows: the chunk parity this warpgroup owns; 128 rows: its half of the tile
     const int tid = threadIdx.x & 127, ctid = threadIdx.x - 128;
     const int w = tid >> 5, lane = tid & 31;
-    const uint32_t a_base = smem_u32(sA), w_base = smem_u32(sW);
-    float* stg = s_stage + cw * FM * F_SROW;
-    int s = cw * NR;  // this warpgroup's ring
+    uint8_t* myA = sA + (WIDE ? (size_t)cw * 2 * a_plane : 0);
+    const uint32_t a_base = smem_u32(myA), w_base = smem_u32(sW);
+    float* stg = s_stage + cw * FM * SROW;
+    float* part = s_part + (WIDE ? cw * 4 * FM : 0);  // [4][64]: partial (chunk parity, slot) of each row
+    const int s0 = WIDE ? 0 : cw * NR;                // this warpgroup's ring
+    int s = s0;
     uint32_t ph = 0;
-    auto advance = [&]() { if (++s == cw * NR + NR) { s = cw * NR; ph ^= 1; } };
-    auto release = [&]() { if (tid == 0) mbar_arrive(&empty[s]); };
+    auto advance = [&]() { if (++s == s0 + NR) { s = s0; ph ^= 1; } };
+    auto release = [&](int slot) { if (tid == 0) mbar_arrive(&empty[slot]); };
+    // the threads that read and write this warpgroup's A operand
+    auto sync_a = [&]() { if constexpr (WIDE) named_bar_sync(2 + cw, 128); else named_bar_sync(1, 256); };
 
     for (int t = blockIdx.x; t < m_tiles; t += gridDim.x) {
-        const int64_t r0 = (int64_t)t * FM;
-        named_bar_sync(1, 256);  // the previous tile's MMAs on A and reads of s_part are done
+        const int64_t rb = (int64_t)t * ROWS + (WIDE ? cw * FM : 0);  // first row of this warpgroup's A
+        if constexpr (!WIDE) named_bar_sync(1, 256);  // the previous tile's MMAs on A and reads of s_part are done
         // ---- stage the layer-0 operand: cat(x, c) -> bf16 hi / lo pairs, 128B-swizzled K blocks ----
         {
             const int kw = p.KB0 * (FK / 2);  // bf16 pairs per row
-            for (int i = ctid; i < FM * kw; i += 256) {
+            const int n_thr = WIDE ? 128 : 256;
+            for (int i = WIDE ? tid : ctid; i < FM * kw; i += n_thr) {
                 const int r = i / kw, k = 2 * (i - r * kw);
-                const int64_t row = r0 + r;
+                const int64_t row = rb + r;
                 float v0 = 0.f, v1 = 0.f;  // masked rows and padded columns stage zeros
                 if (row < p.M) {
                     if (k < p.D) v0 = __ldg(p.x + row * p.ldx + k);
@@ -184,12 +207,12 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                 uint32_t hi, lo;
                 split2_bf16(v0, v1, hi, lo);
                 const uint32_t off = (uint32_t)(k >> 6) * F_TILE + sw128_offset(r, k & 63);
-                *reinterpret_cast<uint32_t*>(sA + off) = hi;
-                *reinterpret_cast<uint32_t*>(sA + a_plane + off) = lo;
+                *reinterpret_cast<uint32_t*>(myA + off) = hi;
+                *reinterpret_cast<uint32_t*>(myA + a_plane + off) = lo;
             }
         }
         fence_proxy_async();  // generic-proxy writes -> visible to the MMAs (async proxy)
-        named_bar_sync(1, 256);
+        sync_a();
 
         // ---- hidden layers: D -> bias, activation -> hi/lo -> A (in place) ----
         for (int l = 0; l < L - 1; ++l) {
@@ -199,22 +222,46 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
             for (int q = 0; q < 4; ++q)
 #pragma unroll
                 for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
-            for (int kb = 0; kb < KB; ++kb) {
-                for (int ch = 0; ch < nch; ++ch) {
-                    if (!((p.kbmask[l][ch] >> kb) & 1u)) continue;
-                    if ((ch & 1) == cw) {
+            if constexpr (WIDE) {
+                // accumulator q = chunk q; one group per tile, its slot released once the next tile is issued
+                int held = -1;
+                for (int kb = 0; kb < KB; ++kb) {
+#pragma unroll
+                    for (int q = 0; q < F_WIDE_MAXKB; ++q) {
+                        if (q >= nch || !((p.kbmask[l][q] >> kb) & 1u)) continue;
                         mbar_wait(&full[s], ph);
-                        tile_mma(acc, ch >> 1, a_base + (uint32_t)kb * F_TILE, a_plane, w_base + (uint32_t)s * F_STAGE, p.n_terms);
-                        release();
+                        const uint32_t a_hi = a_base + (uint32_t)kb * F_TILE, w_tile = w_base + (uint32_t)s * F_STAGE;
+                        wgmma_fence();
+                        wgmma_kblock(acc[q], a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
+                        wgmma_commit();
+                        wgmma_wait1();
+                        if (held >= 0) release(held);
+                        held = s;
                         advance();
                     }
                 }
+                wgmma_wait0();
+                if (held >= 0) release(held);
+#pragma unroll
+                for (int q = 0; q < 4; ++q) acc_fence(acc[q]);
+            } else {
+                for (int kb = 0; kb < KB; ++kb) {
+                    for (int ch = 0; ch < nch; ++ch) {
+                        if (!((p.kbmask[l][ch] >> kb) & 1u)) continue;
+                        if ((ch & 1) == cw) {
+                            mbar_wait(&full[s], ph);
+                            tile_mma(acc, ch >> 1, a_base + (uint32_t)kb * F_TILE, a_plane, w_base + (uint32_t)s * F_STAGE, n_terms);
+                            release(s);
+                            advance();
+                        }
+                    }
+                }
             }
-            named_bar_sync(1, 256);  // both warpgroups are done reading A: overwrite it
+            sync_a();  // every reader of this A operand is done with it: overwrite it
             const float* bias = p.bias[l];
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
-                const int ch = 2 * q + cw;
+                const int ch = WIDE ? q : 2 * q + cw;
                 if (ch >= nch) continue;
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
@@ -233,22 +280,36 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                         uint32_t hi, lo;
                         split2_bf16(v[0], v[1], hi, lo);
                         const uint32_t off = (uint32_t)ch * F_TILE + sw128_offset(r, col);
-                        *reinterpret_cast<uint32_t*>(sA + off) = hi;
-                        *reinterpret_cast<uint32_t*>(sA + a_plane + off) = lo;
+                        *reinterpret_cast<uint32_t*>(myA + off) = hi;
+                        *reinterpret_cast<uint32_t*>(myA + a_plane + off) = lo;
                     }
                 }
             }
             fence_proxy_async();
-            named_bar_sync(1, 256);
+            sync_a();
         }
 
         // ---- last layer: chunk = whole dims -> staged raw parameters -> bijector + ladj per thread ----
         const int r = tid & 63, slot = tid >> 6;  // evaluation: thread = (sample row, share of the chunk's dims)
-        const int64_t row = r0 + r;
+        const int64_t row = rb + r;
         const bool row_ok = row < p.M;
         const float* bias = p.bias[L - 1];
-        float lsum = 0.f;
-        auto finish_dim = [&](int d, float yv, float lj) {
+        // accumulators (+ bias) of output chunk ch -> this warpgroup's staging buffer
+        auto stage_chunk = [&](const float (&a)[32], int ch) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                if (8 * i >= NP) break;
+                const int col = 8 * i + 2 * (lane & 3);
+                const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + ch * FK + col));
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    float* dst = stg + (w * 16 + (lane >> 2) + 8 * hh) * SROW + col;
+                    if (col < NP) dst[0] = a[4 * i + 2 * hh] + bb.x;
+                    if (col + 1 < NP) dst[1] = a[4 * i + 2 * hh + 1] + bb.y;
+                }
+            }
+        };
+        auto finish_dim = [&](float& ls, int d, float yv, float lj) {
             if (p.y) p.y[row * p.ldy + d] = yv;
             if (p.log_prob) {
                 const float mu = p.base_loc ? p.base_loc[d] : 0.f;
@@ -256,36 +317,11 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                 const float u = (yv - mu) / sg;
                 lj += -0.5f * u * u - logf(sg) - kHalfLog2Pi;
             }
-            lsum += lj;
+            ls += lj;
         };
-        for (int ch = 0; ch < p.n_last; ++ch) {
-            const bool mine = (ch & 1) == cw;
-            float acc[4][32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) acc[0][i] = 0.f;
-            for (int kb = 0; kb < nch; ++kb) {
-                if (!((p.kbmask[L - 1][ch] >> kb) & 1u)) continue;
-                if (mine) {
-                    mbar_wait(&full[s], ph);
-                    tile_mma(acc, 0, a_base + (uint32_t)kb * F_TILE, a_plane, w_base + (uint32_t)s * F_STAGE, p.n_terms);
-                    release();
-                    advance();
-                }
-            }
-            if (!mine) continue;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int col = 8 * i + 2 * (lane & 3);
-                const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + ch * FK + col));
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    float* dst = stg + (w * 16 + (lane >> 2) + 8 * hh) * F_SROW + col;
-                    dst[0] = acc[0][4 * i + 2 * hh] + bb.x;
-                    dst[1] = acc[0][4 * i + 2 * hh + 1] + bb.y;
-                }
-            }
-            named_bar_sync(2 + cw, 128);
-            const float* pr = stg + r * F_SROW;
+        // bijector + log-derivative of this thread's dims of staged chunk ch, summed into ls
+        auto eval_chunk = [&](int ch, float& ls) {
+            const float* pr = stg + r * SROW;
             if constexpr (UNI == ZK_UNI_RQS) {
                 if (slot < DPC) {
                     const int d = ch * DPC + slot;
@@ -297,7 +333,7 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                         float yv, lj;
                         Bin b = rqs_select<KT, FAST, false>(pp, KT, xv, p.bound, p.aw, p.ad);
                         rqs_forward_eval<FAST>(b, xv, yv, lj);
-                        finish_dim(d, yv, lj);
+                        finish_dim(ls, d, yv, lj);
                     }
                 }
             } else {
@@ -306,21 +342,88 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                     const int dl = slot * 16 + j, d = ch * DPC + dl;
                     if (d < p.D && row_ok) {
                         const float shift = pr[2 * dl];
-                        const float ls = softclip<FAST>(pr[2 * dl + 1], p.ad);
+                        const float ls_ = softclip<FAST>(pr[2 * dl + 1], p.ad);
                         const float xv = __ldg(p.x + row * p.ldx + d);
-                        finish_dim(d, fmaf(xv, zexp<FAST>(ls), shift), ls);
+                        finish_dim(ls, d, fmaf(xv, zexp<FAST>(ls_), shift), ls_);
                     }
                 }
             }
-            named_bar_sync(2 + cw, 128);  // staging buffer free for the next chunk
+        };
+        if constexpr (WIDE) {
+            // the next tile's inputs are fetched into L2 while this tile's output layer runs
+            {
+                const int64_t nrow = rb + (int64_t)gridDim.x * ROWS + r;
+                if (nrow < p.M) {
+                    const float* src = slot ? p.c + nrow * p.ldc : p.x + nrow * p.ldx;
+                    const int len = slot ? p.C : p.D;
+                    for (int k = 0; k < len; k += 32) prefetch_l2(src + k);
+                }
+            }
+            // a chunk's tiles (at most F_WIDE_MAXKB <= n_stages) are multiplied as one batch of asynchronous MMAs and
+            // released together once they are done.  The bijector runs with no MMAs in flight: its divergent
+            // branches inside a wgmma pipeline stage make ptxas serialize every wgmma of the kernel (C7515).
+            float acc[32];
+            float ls0 = 0.f, ls1 = 0.f;  // partials of the even and of the odd chunks
+            auto out_chunk = [&](int ch, float& ls) {
+#pragma unroll
+                for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+                const int hs = s;
+                int hn = 0;
+                for (int kb = 0; kb < nch; ++kb) {
+                    if (!((p.kbmask[L - 1][ch] >> kb) & 1u)) continue;
+                    mbar_wait(&full[s], ph);
+                    const uint32_t a_hi = a_base + (uint32_t)kb * F_TILE, w_tile = w_base + (uint32_t)s * F_STAGE;
+                    wgmma_fence();
+                    wgmma_kblock(acc, a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
+                    wgmma_commit();
+                    ++hn;
+                    advance();
+                }
+                wgmma_wait0();
+                acc_fence(acc);
+                for (int i = 0; i < hn; ++i) release((hs + i) % NS);
+                stage_chunk(acc, ch);
+                named_bar_sync(2 + cw, 128);
+                eval_chunk(ch, ls);
+                named_bar_sync(2 + cw, 128);  // staging buffer free for the next chunk
+            };
+            for (int ch = 0; ch < p.n_last; ch += 2) {
+                out_chunk(ch, ls0);
+                if (ch + 1 < p.n_last) out_chunk(ch + 1, ls1);
+            }
+            part[slot * FM + r] = ls0;
+            part[(2 + slot) * FM + r] = ls1;
+        } else {
+            float lsum = 0.f;
+            for (int ch = 0; ch < p.n_last; ++ch) {
+                const bool mine = (ch & 1) == cw;
+                float acc[4][32];
+#pragma unroll
+                for (int i = 0; i < 32; ++i) acc[0][i] = 0.f;
+                for (int kb = 0; kb < nch; ++kb) {
+                    if (!((p.kbmask[L - 1][ch] >> kb) & 1u)) continue;
+                    if (mine) {
+                        mbar_wait(&full[s], ph);
+                        tile_mma(acc, 0, a_base + (uint32_t)kb * F_TILE, a_plane, w_base + (uint32_t)s * F_STAGE, n_terms);
+                        release(s);
+                        advance();
+                    }
+                }
+                if (!mine) continue;
+                stage_chunk(acc[0], ch);
+                named_bar_sync(2 + cw, 128);
+                eval_chunk(ch, lsum);
+                named_bar_sync(2 + cw, 128);  // staging buffer free for the next chunk
+            }
+            part[(2 * cw + slot) * FM + r] = lsum;
         }
-        // ---- per-sample sum over the four (warpgroup, share) partials, fixed order ----
-        s_part[(2 * cw + slot) * FM + r] = lsum;
-        named_bar_sync(1, 256);
-        if (ctid < FM) {
-            const int64_t rr = r0 + ctid;
+        // ---- per-sample sum over the four (chunk parity, share) partials, fixed order ----
+        sync_a();
+        const int sr = WIDE ? tid : ctid;
+        if (sr < FM) {
+            const int64_t rr = rb + sr;
             if (rr < p.M) {
-                const float tot = s_part[ctid] + s_part[FM + ctid] + s_part[2 * FM + ctid] + s_part[3 * FM + ctid] +
+                const float tot = part[sr] + part[FM + sr] + part[2 * FM + sr] + part[3 * FM + sr] +
                                   (p.accumulate ? p.ladj[rr] : 0.f);
                 if (p.log_prob) p.log_prob[rr] = tot;
                 else if (p.ladj) p.ladj[rr] = tot;
@@ -329,15 +432,44 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
     }
 }
 
-template <int UNI, int KT>
+template <int UNI, int KT, int ROWS, int NT>
 zk_status launch_fused_t(const FusedParams& p, bool fast, int grid, size_t smem, cudaStream_t st) {
     auto go = [&](auto kern) -> zk_status {
         ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F_SMEM_MAX));
         kern<<<grid, F_THREADS, smem, st>>>(p);
         return check_launch("fused_layer_kernel");
     };
-    if (p.act > 1) return fast ? go(fused_layer_kernel<UNI, KT, true, true>) : go(fused_layer_kernel<UNI, KT, false, true>);
-    return fast ? go(fused_layer_kernel<UNI, KT, true, false>) : go(fused_layer_kernel<UNI, KT, false, false>);
+    if (p.act > 1)
+        return fast ? go(fused_layer_kernel<UNI, KT, true, true, ROWS, NT>) : go(fused_layer_kernel<UNI, KT, false, true, ROWS, NT>);
+    return fast ? go(fused_layer_kernel<UNI, KT, true, false, ROWS, NT>) : go(fused_layer_kernel<UNI, KT, false, false, ROWS, NT>);
+}
+
+template <int UNI, int KT>
+zk_status launch_fused_rows(const FusedParams& p, int rows, bool fast, int grid, size_t smem, cudaStream_t st) {
+    if (rows == 64) return launch_fused_t<UNI, KT, 64, 0>(p, fast, grid, smem, st);
+    return p.n_terms == 3 ? launch_fused_t<UNI, KT, 128, 3>(p, fast, grid, smem, st) : launch_fused_t<UNI, KT, 128, 1>(p, fast, grid, smem, st);
+}
+
+// Row tile and W ring depth of a shape: 128-row tiles when the four accumulators of a consumer hold every
+// hidden chunk (KBA <= 4) and a ring of at least four slots fits beside the two A operands; 64-row tiles
+// otherwise.  The ring gets every byte of shared memory the A operand(s), staging buffers, partials and
+// barriers leave.
+struct FusedPlan {
+    int rows = 0, n_stages = 0;
+    size_t smem = 0;
+};
+FusedPlan fused_plan(int KBA, int univariate, int bins) {
+    const uint32_t srow = (uint32_t)f_srow(fused_dpc(univariate, bins) * fused_p(univariate, bins));
+    for (int rows : {128, 64}) {
+        const uint32_t fixed = 1024u /*alignment slack*/ + (uint32_t)(rows / FM) * 2u * (uint32_t)KBA * F_TILE +
+                               2u * FM * srow * 4u + 4u * (uint32_t)rows * 4u + 2u * F_MAX_STAGES * 8u;
+        if (fixed >= F_SMEM_MAX) continue;
+        int ns = (int)std::min<uint32_t>(F_MAX_STAGES, (F_SMEM_MAX - fixed) / F_STAGE);
+        if (rows == 128 && (KBA > F_WIDE_MAXKB || ns < 4)) continue;
+        if (rows == 64) ns &= ~1;  // two rings of equal depth
+        return {rows, ns, (size_t)ns * F_STAGE + fixed};
+    }
+    return {};
 }
 
 }  // namespace
@@ -369,6 +501,16 @@ bool fused_layer_supported(const zk_mlp* m, int univariate, int bins, int D, int
 
 int fused_layer_kind(const zk_mlp* m, int univariate, int bins, int D, int C) {
     return fused_layer_supported(m, univariate, bins, D, C) ? 1 : 0;
+}
+
+// K blocks of the fused kernel's A operand: the wider of the input and the hidden width
+static int fused_kba(const zk_mlp* m) {
+    return std::max(((const TcPack*)m->tc)->layers[0].Kp / FK, m->dims[1] / FK);
+}
+
+int fused_tile_rows(const zk_mlp* m, int univariate, int bins, int D, int C) {
+    if (!fused_layer_supported(m, univariate, bins, D, C)) return 0;
+    return fused_plan(fused_kba(m), univariate, bins).rows;
 }
 
 namespace {
@@ -540,7 +682,7 @@ zk_status fused_layer_prepare(zk_mlp* m, const uint8_t* const* mask_dev, int uni
 
 zk_status launch_fused_layer(const zk_mlp* m, const FusedLayerArgs& a, cudaStream_t st) {
     ZK_REQUIRE(fused_layer_supported(m, a.univariate, a.bins, a.D, a.C), "fused layer: the conditioner was not prepared for this bijector");
-    ZK_REQUIRE(a.B < ((int64_t)1 << 31) - FM, "fused layer: batch too large for one launch");
+    ZK_REQUIRE(a.B < ((int64_t)1 << 31) - 2 * FM, "fused layer: batch too large for one launch");
     if (a.B == 0) return ZK_OK;
     const TcPack* pk = (const TcPack*)m->tc;
     const FusedPack& f = pk->fused;
@@ -555,7 +697,7 @@ zk_status launch_fused_layer(const zk_mlp* m, const FusedLayerArgs& a, cudaStrea
     p.K0 = a.D + a.C;
     p.KB0 = pk->layers[0].Kp / FK;
     p.H = m->dims[1];
-    p.KBA = std::max(p.KB0, p.H / FK);
+    p.KBA = fused_kba(m);
     p.D = a.D; p.C = a.C;
     p.n_last = f.n_last;
     p.n_terms = pk->n_terms;
@@ -568,15 +710,14 @@ zk_status launch_fused_layer(const zk_mlp* m, const FusedLayerArgs& a, cudaStrea
     const float absL = fabsf(logf(a.slope));
     p.aw = 2.f / absL;
     p.ad = 1.f / absL;
-    // the W rings get every byte of shared memory the A operand and the staging buffers leave
-    const uint32_t fixed = 1024u /*alignment slack*/ + 2u * (uint32_t)p.KBA * F_TILE + F_STAGING_BYTES + F_AUX_BYTES;
-    p.n_stages = (int)std::min<uint32_t>(F_MAX_STAGES, (F_SMEM_MAX - fixed) / F_STAGE) & ~1;
-    ZK_REQUIRE(p.n_stages >= 4, "fused layer: not enough shared memory for the weight rings");
-    const size_t smem = (size_t)p.n_stages * F_STAGE + fixed;
-    const int grid = (int)std::min<int64_t>(ceil_div(a.B, FM), sm_count());
-    if (a.univariate == ZK_UNI_RQS && a.bins == 8) return launch_fused_t<ZK_UNI_RQS, 8>(p, a.fast_math, grid, smem, st);
-    if (a.univariate == ZK_UNI_RQS) return launch_fused_t<ZK_UNI_RQS, 16>(p, a.fast_math, grid, smem, st);
-    return launch_fused_t<ZK_UNI_AFFINE, 0>(p, a.fast_math, grid, smem, st);
+    const FusedPlan plan = fused_plan(p.KBA, a.univariate, a.bins);
+    ZK_REQUIRE(plan.n_stages >= 4, "fused layer: not enough shared memory for the weight rings");
+    p.n_stages = plan.n_stages;
+    const int grid = (int)std::min<int64_t>(ceil_div(a.B, plan.rows), sm_count());
+    if (a.univariate == ZK_UNI_RQS && a.bins == 8)
+        return launch_fused_rows<ZK_UNI_RQS, 8>(p, plan.rows, a.fast_math, grid, plan.smem, st);
+    if (a.univariate == ZK_UNI_RQS) return launch_fused_rows<ZK_UNI_RQS, 16>(p, plan.rows, a.fast_math, grid, plan.smem, st);
+    return launch_fused_rows<ZK_UNI_AFFINE, 0>(p, plan.rows, a.fast_math, grid, plan.smem, st);
 }
 
 }  // namespace zk

@@ -27,6 +27,8 @@ struct FusedLayerArgs {
 bool fused_layer_supported(const zk_mlp* m, int univariate, int bins, int D, int C);
 // which kernel: 0 none, 1 the fused layer kernel (fused_layer.cu)
 int fused_layer_kind(const zk_mlp* m, int univariate, int bins, int D, int C);
+// rows per tile of the fused layer kernel for this layer (64 or 128, from the shape); 0 when it does not run fused
+int fused_tile_rows(const zk_mlp* m, int univariate, int bins, int D, int C);
 // Builds the fused kernel's weight pack for this conditioner (degree-sorted hidden units, zero-tile
 // map); `mask_dev` are the DEVICE mask pointers of zk_mlp_desc (may be null = dense).  No-op when
 // the shape is not supported by the fused kernel.
