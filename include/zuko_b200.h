@@ -51,6 +51,10 @@ typedef void* zk_stream; /* cudaStream_t */
                            (layers only: NCSF; `bound` of the layer is pi) */
 #define ZK_UNI_GAUSS 4  /* GaussianizationTransform, zuko/transforms.py:834-875; phi = (shift[K], scale[K]), inverse by
                            bisection on [-bound, bound] (transforms.py:609-617); element-wise layers only */
+#define ZK_UNI_SOSP 5   /* ShiftedSOSPTransform = SOSPolynomialTransform(a, slope) then AdditiveTransform(constant),
+                           zuko/flows/polynomial.py:23-28, transforms.py:878-963; phi = (a[K][L+1] row-major, constant),
+                           P = K (L + 1) + 1 (K = `bins`, L = `degree`); inverse by bisection on [-bound, bound];
+                           autoregressive layers only */
 /* base distribution of a flow */
 #define ZK_BASE_DIAG_NORMAL 0 /* DiagNormal(loc, scale)    zuko/distributions.py:337-363 */
 #define ZK_BASE_BOX_UNIFORM 1 /* BoxUniform(lower, upper)  zuko/distributions.py:366-396; base_loc = lower, base_scale = upper */
@@ -121,6 +125,17 @@ zk_status zk_gaussianization_forward(const float* x, int64_t ldx, const float* p
 zk_status zk_gaussianization_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B,
                                      int D, int K, float bound, int iterations, float* x, int64_t ldx,
                                      zk_stream stream);
+/* ShiftedSOSPTransform(a, constant, slope) with SOSPolynomialTransform's bound — flows/polynomial.py:23-28,
+ * transforms.py:878-963; phi = (a[K][degree+1] row-major, constant) per pair, 1 <= K, 0 <= degree <= 15,
+ * K (degree + 1) + 1 <= 1024.  Forward: y = x sum_i w_i g(t_i x) + constant (degree + 1 Gauss-Legendre nodes)
+ * and ladj = log g(x).  Inverse: `iterations` bisection steps on [-bound, bound] of y - constant; a y beyond
+ * the range of f returns +-(bound - half the final interval), as the reference does. */
+zk_status zk_sosp_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
+                          int K, int degree, float bound, float slope, float* y, int64_t ldy, float* ladj,
+                          int accumulate, zk_stream stream);
+zk_status zk_sosp_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B, int D,
+                          int K, int degree, float bound, float slope, int iterations, float* x, int64_t ldx,
+                          zk_stream stream);
 /* SoftclipTransform(bound)                       — transforms.py:299-316 */
 zk_status zk_softclip_forward(const float* x, int64_t ldx, int64_t B, int D, float bound, float* y,
                               int64_t ldy, float* ladj, int accumulate, zk_stream stream);
@@ -195,8 +210,8 @@ typedef struct {
     int features;   /* D */
     int context;    /* C (0 = unconditional) */
     int univariate; /* ZK_UNI_* (autoregressive / coupling / elementwise) */
-    int bins;       /* K for ZK_UNI_RQS, mixture components K for ZK_UNI_GAUSS */
-    float bound;    /* spline bound B (5.0), softclip bound or Gaussianization bisection bound (10.0) */
+    int bins;       /* K for ZK_UNI_RQS, mixture components K for ZK_UNI_GAUSS, polynomials K for ZK_UNI_SOSP */
+    float bound;    /* spline bound B (5.0), softclip bound or the bisection bound of ZK_UNI_GAUSS / ZK_UNI_SOSP (10.0) */
     float slope;    /* minimum slope (1e-3) */
     int passes;     /* autoregressive: number of inverse sweeps (transforms.py:994-1000) */
     const int64_t* order;         /* host (D): autoregressive order classes (MaskedAutoregressiveTransform.order,
@@ -205,7 +220,8 @@ typedef struct {
     const zk_mlp_desc* hyper;     /* conditioner; NULL for parameter-free / shared-table layers */
     const float* phi;             /* DEVICE (D, P) shared table: elementwise without context */
     const float* rotation;        /* DEVICE (D, D) R for ZK_LAYER_ROTATION */
-    int iterations;               /* ZK_UNI_GAUSS: bisection steps of the inverse, ceil(log2(2 bound / eps)) (>= 1) */
+    int iterations;               /* ZK_UNI_GAUSS / ZK_UNI_SOSP: bisection steps of the inverse, ceil(log2(2 bound / eps)) (>= 1) */
+    int degree;                   /* ZK_UNI_SOSP: polynomial degree L (0 .. 15) */
 } zk_layer_desc;
 
 zk_status zk_layer_create(const zk_layer_desc* desc, zk_layer** out);
@@ -342,6 +358,11 @@ zk_status zk_gaussianization_backward(const float* x, int64_t ldx, const float* 
                                       int D, int K, const float* grad_y, int64_t ldgy, const float* grad_ladj,
                                       float* grad_x, int64_t ldgx, float* grad_phi, void* workspace,
                                       size_t workspace_bytes, zk_stream stream);
+/* same for ShiftedSOSPTransform (flows/polynomial.py:23-28, transforms.py:878-963), P = K (degree + 1) + 1 */
+zk_status zk_sosp_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
+                           int K, int degree, float bound, float slope, const float* grad_y, int64_t ldgy,
+                           const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi, void* workspace,
+                           size_t workspace_bytes, zk_stream stream);
 /* SoftclipTransform (transforms.py:299-316) */
 zk_status zk_softclip_backward(const float* x, int64_t ldx, int64_t B, int D, float bound,
                                const float* grad_y, int64_t ldgy, const float* grad_ladj,
@@ -417,7 +438,8 @@ int zk_set_tc_backward(int on);
 
 /* Transcendental arithmetic of the bijector kernels: 1 (default) = MUFU rcp / ex2 / lg2
  * approximations, 0 = IEEE division + expf / logf (erf / erfc / erfcinv of the Gaussianization
- * bijector are IEEE-library calls in both settings).  Process-wide; returns the previous
+ * bijector are IEEE-library calls in both settings; the sum-of-squares polynomial bijector uses the
+ * approximation only for the log of its ladj).  Process-wide; returns the previous
  * value.  Both settings meet the 1e-5 parity bar on the BASELINE configs (tests/). */
 int zk_set_fast_math(int on);
 /* 1 (default): an autoregressive layer whose conditioner fits the fused kernel (hidden widths

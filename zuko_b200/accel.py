@@ -51,6 +51,8 @@ _ENGINE_CALLABLES = {
     "MonotonicAffineTransform": _T.MonotonicAffineTransform,
     "MonotonicRQSTransform": _T.MonotonicRQSTransform,
     "SoftclipTransform": _T.SoftclipTransform,
+    "ShiftedSOSPTransform": _T.ShiftedSOSPTransform,
+    "SOSPolynomialTransform": _T.SOSPolynomialTransform,
     "PermutationTransform": _T.PermutationTransform,
     "RotationTransform": _T.RotationTransform,
 }

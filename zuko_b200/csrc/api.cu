@@ -130,6 +130,26 @@ zk_status zk_gaussianization_inverse(const float* y, int64_t ldy, const float* p
     return launch_univariate(a, (cudaStream_t)stream);
 }
 
+zk_status zk_sosp_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
+                          int K, int degree, float bound, float slope, float* y, int64_t ldy, float* ladj,
+                          int accumulate, zk_stream stream) {
+    UniArgs a;
+    a.univariate = ZK_UNI_SOSP; a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = phi_ld; a.B = B; a.D = D;
+    a.K = K; a.degree = degree; a.bound = bound; a.slope = slope; a.y = y; a.ldy = ldy; a.ladj = ladj;
+    a.accumulate = accumulate; a.fast_math = g_fast_math.load() != 0;
+    return launch_univariate(a, (cudaStream_t)stream);
+}
+
+zk_status zk_sosp_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B, int D,
+                          int K, int degree, float bound, float slope, int iterations, float* x, int64_t ldx,
+                          zk_stream stream) {
+    UniArgs a;
+    a.univariate = ZK_UNI_SOSP; a.inverse = true; a.x = y; a.ldx = ldy; a.phi = phi; a.phi_ld = phi_ld;
+    a.B = B; a.D = D; a.K = K; a.degree = degree; a.bound = bound; a.slope = slope; a.iters = iterations;
+    a.y = x; a.ldy = ldx; a.fast_math = g_fast_math.load() != 0;
+    return launch_univariate(a, (cudaStream_t)stream);
+}
+
 zk_status zk_softclip_forward(const float* x, int64_t ldx, int64_t B, int D, float bound, float* y,
                               int64_t ldy, float* ladj, int accumulate, zk_stream stream) {
     return launch_softclip(x, ldx, B, D, bound, false, y, ldy, ladj, accumulate, (cudaStream_t)stream);
@@ -324,12 +344,14 @@ static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
         l->circ = true;
     }
     l->K = d->bins; l->bound = d->bound; l->slope = d->slope; l->passes = d->passes; l->iters = d->iterations;
+    l->degree = d->degree;
     ZK_REQUIRE(l->D >= 1, "layer_create: features=%d", l->D);
     ZK_REQUIRE(l->C >= 0, "layer_create: context=%d", l->C);
     const bool has_uni = (l->kind == ZK_LAYER_AUTOREGRESSIVE || l->kind == ZK_LAYER_COUPLING ||
                           l->kind == ZK_LAYER_ELEMENTWISE);
     if (has_uni) {
-        ZK_REQUIRE(l->uni == ZK_UNI_AFFINE || l->uni == ZK_UNI_RQS || l->uni == ZK_UNI_GAUSS, "layer_create: univariate=%d", d->univariate);
+        ZK_REQUIRE(l->uni == ZK_UNI_AFFINE || l->uni == ZK_UNI_RQS || l->uni == ZK_UNI_GAUSS || l->uni == ZK_UNI_SOSP,
+                   "layer_create: univariate=%d", d->univariate);
         if (l->uni == ZK_UNI_GAUSS) {  // the bisection inverse is element-wise only (flows/gaussianization.py:97-155)
             if (l->kind != ZK_LAYER_ELEMENTWISE)
                 return fail(ZK_EUNSUPPORTED, "layer_create: the Gaussianization bijector is supported in element-wise layers only");
@@ -337,9 +359,17 @@ static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
             ZK_REQUIRE(l->bound > 0.f, "layer_create: bisection bound=%g", (double)l->bound);
             ZK_REQUIRE(l->iters >= 1 && l->iters <= 64, "layer_create: bisection iterations=%d (must be in [1, 64])", l->iters);
         }
+        if (l->uni == ZK_UNI_SOSP) {  // the bisection runs in autoregressive layers only (flows/polynomial.py:31-76)
+            if (l->kind != ZK_LAYER_AUTOREGRESSIVE)
+                return fail(ZK_EUNSUPPORTED, "layer_create: the SOSP bijector is supported in autoregressive layers only");
+            ZK_REQUIRE(sosp_shape_ok(l->K, l->degree),
+                       "layer_create: SOSP polynomials=%d degree=%d (degree <= 15, K (degree + 1) + 1 <= 1024)", l->K, l->degree);
+            ZK_REQUIRE(l->bound > 0.f, "layer_create: bisection bound=%g", (double)l->bound);
+            ZK_REQUIRE(l->iters >= 1 && l->iters <= 64, "layer_create: bisection iterations=%d (must be in [1, 64])", l->iters);
+        }
         if (l->uni == ZK_UNI_RQS) ZK_REQUIRE(l->K >= 1 && l->K <= 1024, "layer_create: bins=%d", l->K);
         ZK_REQUIRE(l->slope > 0.f && l->slope < 1.f, "layer_create: slope=%g", (double)l->slope);
-        l->P = (l->uni == ZK_UNI_RQS) ? 3 * l->K - 1 : (l->uni == ZK_UNI_GAUSS ? 2 * l->K : 2);
+        l->P = uni_param_count(l->uni, l->K, l->degree);
     }
     switch (l->kind) {
         case ZK_LAYER_AUTOREGRESSIVE: {
@@ -356,7 +386,7 @@ static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
             {
                 int T = 0;
                 size_t smem = 0;
-                ZK_TRY(ar_inverse_pack(l->hyper, d->hyper->mask, d->order, l->D, l->C, l->uni, l->K, l->passes, &l->inv));
+                ZK_TRY(ar_inverse_pack(l->hyper, d->hyper->mask, d->order, l->D, l->C, l->uni, l->K, l->degree, l->passes, &l->inv));
                 if (l->inv && !ar_inverse_threads(l->inv, &T, &smem)) {  // state too large: use the sweeps
                     ar_inverse_free(l->inv);
                     l->inv = nullptr;
@@ -537,7 +567,7 @@ zk_status layer_forward_impl(const zk_layer* l, const float* x, int64_t ldx, con
     ZK_REQUIRE(l->C == 0 || c != nullptr, "layer needs a context of %d features", l->C);
     Arena ar(ws, ws_bytes);
     UniArgs a;
-    a.univariate = l->uni; a.B = B; a.K = l->K; a.bound = l->bound; a.slope = l->slope;
+    a.univariate = l->uni; a.B = B; a.K = l->K; a.degree = l->degree; a.bound = l->bound; a.slope = l->slope;
     a.ladj = ladj; a.accumulate = accumulate; a.log_prob = log_prob; a.base_loc = loc;
     a.base_scale = scale; a.fast_math = g_fast_math.load() != 0; a.circular = l->circ;
     switch (l->kind) {
@@ -619,7 +649,7 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
     ZK_REQUIRE(l->C == 0 || c != nullptr, "layer needs a context of %d features", l->C);
     Arena ar(ws, ws_bytes);
     UniArgs a;
-    a.univariate = l->uni; a.inverse = true; a.B = B; a.K = l->K; a.bound = l->bound; a.iters = l->iters;
+    a.univariate = l->uni; a.inverse = true; a.B = B; a.K = l->K; a.degree = l->degree; a.bound = l->bound; a.iters = l->iters;
     a.slope = l->slope; a.fast_math = g_fast_math.load() != 0; a.circular = l->circ;
     switch (l->kind) {
         case ZK_LAYER_AUTOREGRESSIVE: {
@@ -635,7 +665,7 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
                     int T = 0;
                     size_t smem = 0;
                     ZK_TRY(ar_inverse_pack(ml->hyper, ml->hyper->mask.data(), ml->order.empty() ? nullptr : ml->order.data(), ml->D,
-                                           ml->C, ml->uni, ml->K, ml->passes, &ml->inv));
+                                           ml->C, ml->uni, ml->K, ml->degree, ml->passes, &ml->inv));
                     if (ml->inv && !ar_inverse_threads(ml->inv, &T, &smem)) {
                         ar_inverse_free(ml->inv);
                         ml->inv = nullptr;
@@ -646,7 +676,7 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
             if (l->inv && g_fused.load()) {  // same fixed point, every weight visited once (ar_inverse.cu)
                 ArInvArgs ia;
                 ia.y = y; ia.ldy = ldy; ia.c = c; ia.ldc = ldc; ia.B = B; ia.x = x; ia.ldx = ldx;
-                ia.bound = l->bound; ia.slope = l->slope; ia.fast = g_fast_math.load() != 0; ia.circular = l->circ;
+                ia.bound = l->bound; ia.slope = l->slope; ia.iters = l->iters; ia.fast = g_fast_math.load() != 0; ia.circular = l->circ;
                 if (ladj) {
                     ia.ladj = ladj; ia.accumulate = accumulate; ia.base = base_lp; ia.base_loc = base_loc; ia.base_scale = base_scale;
                     ia.as_inverse_member = as_member;

@@ -310,7 +310,7 @@ zk_status layer_backward_impl(const zk_layer* l, const float* x, int64_t ldx, co
     ZK_REQUIRE(l->C == 0 || c != nullptr, "layer needs a context of %d features", l->C);
     Arena ar(ws, ws_bytes);
     UniBwdArgs u;
-    u.univariate = l->uni; u.B = B; u.K = l->K; u.bound = l->bound; u.slope = l->slope; u.circular = l->circ;
+    u.univariate = l->uni; u.B = B; u.K = l->K; u.degree = l->degree; u.bound = l->bound; u.slope = l->slope; u.circular = l->circ;
     u.fast_math = g_fast_math.load() != 0;
     u.x = x; u.ldx = ldx; u.gy = gy; u.ldgy = ldgy; u.gl = gl; u.gx = gx; u.ldgx = ldgx;
     switch (l->kind) {
@@ -611,11 +611,11 @@ zk_status flow_inverse_backward_chunk(const zk_flow_desc* f, const float* x, int
 zk_status uni_backward_entry(int uni, const float* x, int64_t ldx, const float* phi, int64_t phi_ld,
                              int64_t B, int D, int K, float bound, float slope, const float* gy,
                              int64_t ldgy, const float* gl, float* gx, int64_t ldgx, float* gphi,
-                             void* ws, size_t ws_bytes, cudaStream_t st) {
+                             void* ws, size_t ws_bytes, cudaStream_t st, int degree = 0) {
     ZK_REQUIRE(x && phi && B >= 0 && D > 0, "univariate backward: bad arguments");
-    const int P = (uni == ZK_UNI_RQS) ? 3 * K - 1 : (uni == ZK_UNI_GAUSS ? 2 * K : 2);
+    const int P = uni_param_count(uni, K, degree);
     UniBwdArgs u;
-    u.univariate = uni; u.K = K; u.bound = bound; u.slope = slope; u.D = D;
+    u.univariate = uni; u.K = K; u.degree = degree; u.bound = bound; u.slope = slope; u.D = D;
     u.fast_math = g_fast_math.load() != 0;
     u.phi = phi; u.phi_ld = phi_ld;
     if (phi_ld != 0 || gphi == nullptr) {
@@ -673,6 +673,15 @@ zk_status zk_gaussianization_backward(const float* x, int64_t ldx, const float* 
     ZK_REQUIRE(K >= 1 && K <= 1024, "gaussianization backward: components must be in [1, 1024], got %d", K);
     return uni_backward_entry(ZK_UNI_GAUSS, x, ldx, phi, phi_ld, B, D, K, 10.f, 1e-3f, grad_y, ldgy, grad_ladj,
                               grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+zk_status zk_sosp_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
+                           int K, int degree, float bound, float slope, const float* grad_y, int64_t ldgy,
+                           const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi, void* ws,
+                           size_t ws_bytes, zk_stream stream) {
+    ZK_REQUIRE(sosp_shape_ok(K, degree), "sosp backward: polynomials %d / degree %d out of range", K, degree);
+    return uni_backward_entry(ZK_UNI_SOSP, x, ldx, phi, phi_ld, B, D, K, bound, slope, grad_y, ldgy, grad_ladj,
+                              grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream, degree);
 }
 
 zk_status zk_softclip_backward(const float* x, int64_t ldx, int64_t B, int D, float bound,

@@ -49,7 +49,8 @@ inline zk_status dev_copy_from_host(const T* host, size_t n, T** out) {
 // ===========================================================================
 struct zk_layer {
     int kind = 0, D = 0, C = 0, uni = 0, K = 0, P = 0, passes = 0;
-    int iters = 0;                 // ZK_UNI_GAUSS: bisection steps of the inverse
+    int iters = 0;                 // ZK_UNI_GAUSS / ZK_UNI_SOSP: bisection steps of the inverse
+    int degree = 0;                // ZK_UNI_SOSP: polynomial degree (K = polynomials)
     float bound = 5.f, slope = 1e-3f;
     bool circ = false;             // ZK_UNI_CRQS: CircularShiftTransform(bound) in front of the spline
     zk_mlp* hyper = nullptr;       // owned

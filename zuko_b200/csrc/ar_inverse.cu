@@ -10,8 +10,9 @@
 //   step p = 0 .. passes-1:
 //     every hidden unit whose inputs became final at step p is computed;
 //     the P parameter rows of every dim of class p are computed from the last hidden layer;
-//     the inverse bijector (transforms.py:534-548 / 443-444) yields x_d, which is stored and
-//     becomes an input of the later steps.
+//     the inverse bijector (transforms.py:534-548 / 443-444, or the SOSP bisection of
+//     transforms.py:609-617 in registers) yields x_d, which is stored and becomes an input of the
+//     later steps.
 //
 // This visits every weight once instead of `passes` times and reproduces the reference's fixed
 // point up to summation order (SURVEY §3.2, §7.2).  The same sweep also yields what
@@ -46,7 +47,7 @@
 namespace zk {
 
 struct ArInvPack {
-    int D = 0, C = 0, P = 0, uni = 0, bins = 0, passes = 0, act = 1;
+    int D = 0, C = 0, P = 0, uni = 0, bins = 0, degree = 0, passes = 0, act = 1;
     int n_linear = 0;
     std::vector<int> dims;         // n_linear + 1
     std::vector<int> sec_off;      // state section offsets (floats): IN, H1 .. H_{L-1}, end
@@ -81,6 +82,7 @@ struct InvParams {
     int base;          // 1: also add DiagNormal(loc, scale).log_prob of the input y (distributions.py:129-138); 2: of the output x
     float sign;        // +1: accumulate the forward ladj at the solution; -1: the layer is an inverted flow member
     const float* base_loc; const float* base_scale;
+    sosp::Const sosp;  // SOSP: bisection and pre-scaled quadrature of the default shape
 };
 
 // two fp32 FMAs on a pair (fmaf rounding)
@@ -124,7 +126,7 @@ __device__ __forceinline__ void tile_dot(const float* __restrict__ w, const floa
 //           then per dim ONE block of its PT tiles: K x (PT * 8) weights k-major + PT * 8 biases
 template <int UNI, int KT, bool FAST, int R, bool GACT>
 __global__ void __launch_bounds__(256) ar_inverse_kernel(const InvParams p) {
-    constexpr int P = (UNI == ZK_UNI_RQS) ? 3 * KT - 1 : 2;
+    constexpr int P = (UNI == ZK_UNI_RQS) ? 3 * KT - 1 : (UNI == ZK_UNI_SOSP ? sosp::kDefP : 2);
     constexpr int PT = (P + TILE - 1) / TILE;  // tiles per dim
     extern __shared__ __align__(16) float state[];  // [state_floats][S], S = R * T samples
     const int T = blockDim.x;
@@ -283,6 +285,9 @@ __global__ void __launch_bounds__(256) ar_inverse_kernel(const InvParams p) {
                         float y2;
                         rqs_forward_eval<FAST>(b, xv, y2, lj);  // ladj of the forward map at the solution
                         if (p.circ) xv = circ_shift(xv, p.bound);  // inverse of flows/spline.py:68-71
+                    } else if constexpr (UNI == ZK_UNI_SOSP) {
+                        xv = sosp::inverse<KT>(phi[j], p.sosp, yv[j]);
+                        lj = zlog<FAST>(sosp::g<KT>(phi[j], p.sosp, xv));  // ladj of the forward map at the solution
                     } else {
                         const float ls = softclip<FAST>(phi[j][1], p.ad);
                         xv = zdiv<FAST>(yv[j] - phi[j][0], zexp<FAST>(ls));
@@ -316,13 +321,17 @@ zk_status launch_inv_t(const InvParams& p, bool fast, int R, int grid, int T, si
         kern<<<grid, T, smem, st>>>(p);
         return check_launch("ar_inverse_kernel");
     };
+    constexpr bool kTwo = UNI != ZK_UNI_SOSP;  // SOSP: one sample per thread only (inv_geometry)
     if (p.act != 1) {  // general activation: one instantiation per sample tiling (IEEE math in the activation)
-        if (R == 2) return fast ? go(ar_inverse_kernel<UNI, KT, true, 2, true>) : go(ar_inverse_kernel<UNI, KT, false, 2, true>);
+        if constexpr (kTwo)
+            if (R == 2) return fast ? go(ar_inverse_kernel<UNI, KT, true, 2, true>) : go(ar_inverse_kernel<UNI, KT, false, 2, true>);
         return fast ? go(ar_inverse_kernel<UNI, KT, true, 1, true>) : go(ar_inverse_kernel<UNI, KT, false, 1, true>);
     }
-    if (R == 2) {
-        if (fast) return go(ar_inverse_kernel<UNI, KT, true, 2, false>);
-        return go(ar_inverse_kernel<UNI, KT, false, 2, false>);
+    if constexpr (kTwo) {
+        if (R == 2) {
+            if (fast) return go(ar_inverse_kernel<UNI, KT, true, 2, false>);
+            return go(ar_inverse_kernel<UNI, KT, false, 2, false>);
+        }
     }
     if (fast) return go(ar_inverse_kernel<UNI, KT, true, 1, false>);
     return go(ar_inverse_kernel<UNI, KT, false, 1, false>);
@@ -338,7 +347,8 @@ bool inv_geometry(const ArInvPack* pk, int* threads, int* per_thread, size_t* sm
     auto set = [&](int T, int R) { *threads = T; *per_thread = R; *smem = per_sample * T * R + wbytes; return true; };
     if (const char* e = getenv("ZK_INV_GEOM")) {
         int T = 0, R = 0;
-        if (sscanf(e, "%dx%d", &T, &R) == 2 && (R == 1 || R == 2) && T >= 32 && T <= 256 && T % 32 == 0 && fits(T, R)) return set(T, R);
+        const bool r2 = pk->uni != ZK_UNI_SOSP;  // SOSP: R = 2 would spill (two register bisections); not compiled
+        if (sscanf(e, "%dx%d", &T, &R) == 2 && (R == 1 || (R == 2 && r2)) && T >= 32 && T <= 256 && T % 32 == 0 && fits(T, R)) return set(T, R);
     }
     // two CTAs of 128 samples per SM when they fit (8 warps hide the FMA / LDS latencies of the dot
     // products far better than 4), else one CTA with as many samples as shared memory holds
@@ -359,14 +369,16 @@ void ar_inverse_free(ArInvPack* pk) {
 }
 
 zk_status ar_inverse_pack(const zk_mlp* m, const uint8_t* const* mask_dev, const int64_t* order, int D, int C,
-                          int uni, int bins, int passes, ArInvPack** out) {
+                          int uni, int bins, int degree, int passes, ArInvPack** out) {
     *out = nullptr;
     const int L = m->n_linear;
     if (!order || L < 1 || L > 7) return ZK_OK;
     if (!m->plain) return ZK_OK;  // residual blocks use the sweeps
     if (uni == ZK_UNI_RQS && bins != 8 && bins != 16) return ZK_OK;
+    if (uni == ZK_UNI_SOSP && (bins != sosp::kDefK || degree != sosp::kDefL)) return ZK_OK;  // compiled for P = 16 only
+    if (uni != ZK_UNI_RQS && uni != ZK_UNI_AFFINE && uni != ZK_UNI_SOSP) return ZK_OK;
     if (m->dims[0] != D + C) return ZK_OK;
-    const int P = (uni == ZK_UNI_RQS) ? 3 * bins - 1 : 2;
+    const int P = uni_param_count(uni, bins, degree);
     if (m->dims[L] != D * P) return ZK_OK;
     for (int d = 0; d < D; ++d)
         if (order[d] < 0 || order[d] >= passes) return ZK_OK;
@@ -404,7 +416,7 @@ zk_status ar_inverse_pack(const zk_mlp* m, const uint8_t* const* mask_dev, const
             if (ready[L - 1][d * P + q] > order[d]) return ZK_OK;  // not a pure order-class structure
 
     ArInvPack* pk = new ArInvPack();
-    pk->D = D; pk->C = C; pk->P = P; pk->uni = uni; pk->bins = bins; pk->passes = passes; pk->n_linear = L;
+    pk->D = D; pk->C = C; pk->P = P; pk->uni = uni; pk->bins = bins; pk->degree = degree; pk->passes = passes; pk->n_linear = L;
     pk->act = m->act;
     pk->dims = m->dims;
     int off = 0;
@@ -565,10 +577,15 @@ zk_status launch_ar_inverse(const ArInvPack* pk, const ArInvArgs& a, cudaStream_
     p.ladj = a.ladj; p.accumulate = a.accumulate; p.base = a.base ? (a.as_inverse_member ? 2 : 1) : 0;
     p.sign = a.as_inverse_member ? -1.f : 1.f;
     p.base_loc = a.base_loc; p.base_scale = a.base_scale;
+    if (pk->uni == ZK_UNI_SOSP) p.sosp = sosp::make_const(pk->bins, pk->degree, a.bound, a.slope, a.iters);
     const int64_t grid = ceil_div(a.B, (int64_t)T * R);
     ZK_REQUIRE(grid <= 0x7fffffff, "ar_inverse: batch too large for one launch");
     if (pk->uni == ZK_UNI_RQS && pk->bins == 8) return launch_inv_t<ZK_UNI_RQS, 8>(p, a.fast, R, (int)grid, T, smem, st);
     if (pk->uni == ZK_UNI_RQS && pk->bins == 16) return launch_inv_t<ZK_UNI_RQS, 16>(p, a.fast, R, (int)grid, T, smem, st);
+    if (pk->uni == ZK_UNI_SOSP) {
+        ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "ar_inverse: bisection steps must be in [1, 64], got %d", a.iters);
+        return launch_inv_t<ZK_UNI_SOSP, sosp::kDefK>(p, a.fast, R, (int)grid, T, smem, st);
+    }
     return launch_inv_t<ZK_UNI_AFFINE, 0>(p, a.fast, R, (int)grid, T, smem, st);
 }
 

@@ -30,6 +30,15 @@ struct UniBwdParams {
     int rows_per_tile;
     int circ;
 };
+// SOSP kernels also take the shape and the pre-scaled quadrature.  A type of their own: appending the
+// table to UniBwdParams changes the register allocation of the RQS and Gaussianization instantiations.
+struct SospBwdParams : UniBwdParams {
+    sosp::Const sosp;
+};
+template <int UNI>
+struct BwdParamsFor { using type = UniBwdParams; };
+template <>
+struct BwdParamsFor<ZK_UNI_SOSP> { using type = SospBwdParams; };
 
 __device__ __forceinline__ float circ_shift_b(float x, float bound) {  // bijector_math.cuh:circ_shift
     const float m = 2.f * bound;
@@ -42,7 +51,7 @@ __device__ __forceinline__ float circ_shift_b(float x, float bound) {  // biject
 // pair rewrites its P slots with the parameter gradients, and the tile is written back with
 // coalesced stores (per-sample gradients (B, D*P); a shared table is reduced by the caller).
 template <int UNI, int KT, bool FAST>
-__global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const UniBwdParams a) {
+__global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const typename BwdParamsFor<UNI>::type a) {
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x;
     const int64_t r0 = (int64_t)blockIdx.x * a.rows_per_tile;
@@ -79,6 +88,15 @@ __global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const UniBwdParams
             float yv, lj;
             bij::gauss_forward_eval<KT, FAST>(pp, a.K, xv, yv, lj);
             bijgrad::gauss_backward_pair<FAST>(pp, KT > 0 ? KT : a.K, xv, yv, gyv, glv, gxv, out);
+        } else if constexpr (UNI == ZK_UNI_SOSP) {
+            if constexpr (KT > 0) {  // register copy of the parameters; out may alias pp
+                float ar[sosp::kDefP];
+#pragma unroll
+                for (int q = 0; q < sosp::kDefP; ++q) ar[q] = pp[q];
+                sosp::backward_pair<KT>(ar, a.sosp, xv, gyv, glv, gxv, out);
+            } else {
+                sosp::backward_pair<0>(pp, a.sosp, xv, gyv, glv, gxv, out);
+            }
         } else {
             bijgrad::affine_backward_pair(pp, xv, gyv, glv, a.ad, gxv, out);
         }
@@ -301,14 +319,15 @@ int wgrad_slices_max(int N, int K) {
 }
 
 template <int UNI, int KT>
-zk_status launch_uni_bwd_t(const UniBwdParams& p, bool fast, int grid, size_t smem, cudaStream_t st) {
+zk_status launch_uni_bwd_t(const typename BwdParamsFor<UNI>::type& p, bool fast, int grid, size_t smem, cudaStream_t st) {
     auto go = [&](auto kern) -> zk_status {
         if (smem > 40 * 1024)
             ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, kBwdThreads, smem, st>>>(p);
         return check_launch("uni_bwd_kernel");
     };
-    if (fast && UNI != ZK_UNI_AFFINE) return go(uni_bwd_kernel<UNI, KT, true>);  // affine: one expf per pair, not worth a variant
+    // affine: one expf per pair, not worth a variant; SOSP: no transcendental in its reverse mode
+    if (fast && UNI != ZK_UNI_AFFINE && UNI != ZK_UNI_SOSP) return go(uni_bwd_kernel<UNI, KT, true>);
     return go(uni_bwd_kernel<UNI, KT, false>);
 }
 
@@ -318,16 +337,18 @@ zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
     ZK_REQUIRE(a.B >= 0 && a.D > 0, "univariate backward: bad shape B=%lld D=%d", (long long)a.B, a.D);
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate backward: null input");
-    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS,
+    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS ||
+                   a.univariate == ZK_UNI_SOSP,
                "univariate backward: unknown kind %d", a.univariate);
-    int P = 2;
     if (a.univariate == ZK_UNI_RQS) {
         ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "rqs backward: bins must be in [1, 1024], got %d", a.K);
-        P = 3 * a.K - 1;
     } else if (a.univariate == ZK_UNI_GAUSS) {
         ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "gaussianization backward: components must be in [1, 1024], got %d", a.K);
-        P = 2 * a.K;
+    } else if (a.univariate == ZK_UNI_SOSP) {
+        ZK_REQUIRE(sosp_shape_ok(a.K, a.degree), "sosp backward: polynomials %d / degree %d out of range", a.K, a.degree);
+        ZK_REQUIRE(a.bound > 0.f, "sosp backward: bound must be positive");
     }
+    const int P = uni_param_count(a.univariate, a.K, a.degree);
     ZK_REQUIRE(a.phi_ld == 0 || a.phi_ld >= (int64_t)a.D * P, "univariate backward: phi_ld too small");
     ZK_REQUIRE(a.slope > 0.f && a.slope < 1.f, "univariate backward: slope must be in (0, 1)");
     ZK_REQUIRE(!(a.phi_ld == 0 && a.gphi == a.phi), "univariate backward: gphi cannot alias a shared table");
@@ -359,6 +380,14 @@ zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
             case 16: return launch_uni_bwd_t<ZK_UNI_GAUSS, 16>(p, a.fast_math, (int)grid, smem, stream);
             default: return launch_uni_bwd_t<ZK_UNI_GAUSS, 0>(p, a.fast_math, (int)grid, smem, stream);
         }
+    }
+    if (a.univariate == ZK_UNI_SOSP) {
+        SospBwdParams sp;
+        static_cast<UniBwdParams&>(sp) = p;
+        sp.sosp = sosp::make_const(a.K, a.degree, a.bound, a.slope, 0);
+        if (a.K == sosp::kDefK && a.degree == sosp::kDefL)
+            return launch_uni_bwd_t<ZK_UNI_SOSP, sosp::kDefK>(sp, a.fast_math, (int)grid, smem, stream);
+        return launch_uni_bwd_t<ZK_UNI_SOSP, 0>(sp, a.fast_math, (int)grid, smem, stream);
     }
     switch (a.K) {
         case 8: return launch_uni_bwd_t<ZK_UNI_RQS, 8>(p, a.fast_math, (int)grid, smem, stream);

@@ -3,6 +3,7 @@
 #pragma once
 
 #include "common.cuh"
+#include "sosp_math.cuh"
 
 namespace zk {
 namespace bij {
@@ -292,16 +293,11 @@ __device__ __forceinline__ float gauss_inverse_eval(const float* __restrict__ p,
     const float cK = (1.f - kGaussFloor) / (float)K;
     const bool upper = y >= 0.f;
     const float target = erfcf(fabsf(y) * kRsqrt2);
-    float lo = -bound, hi = bound;
-    for (int it = 0; it < iters; ++it) {
-        const float m = 0.5f * (lo + hi);
+    return bisect(bound, iters, [&](float m) {
         float sp, sn;
         gauss_tails<KT, FAST>(p, K, sreg, m, sp, sn);
-        const bool below = upper ? (fmaf(cK, sp, kGaussFloor) > target) : (fmaf(cK, sn, kGaussFloor) < target);
-        lo = below ? m : lo;
-        hi = below ? hi : m;
-    }
-    return 0.5f * (lo + hi);
+        return upper ? (fmaf(cK, sp, kGaussFloor) > target) : (fmaf(cK, sn, kGaussFloor) < target);
+    });
 }
 
 

@@ -7,7 +7,9 @@
 // and the ~10 of MonotonicAffineTransform (zuko/transforms.py:426-446), and
 // GaussianizationTransform (zuko/transforms.py:834-875): K erfc terms and the closed-form
 // ladj instead of the reference's autograd call per forward (transforms.py:623-637), and its
-// bisection inverse (transforms.py:609-617, utils.py:159-183) run in registers.
+// bisection inverse (transforms.py:609-617, utils.py:159-183) run in registers, and the
+// sum-of-squares polynomial bijector of SOSPF (flows/polynomial.py:23-28, sosp_math.cuh): its
+// Gauss-Legendre forward, log g(x), and the same bisection on y - constant.
 //
 // Data movement: a CTA owns a tile of R consecutive sample rows.  Their phi block is
 // one contiguous range of R*D*P floats in HBM; it is staged into shared memory with a
@@ -49,7 +51,35 @@ struct UniParams {
     int circ;      // RQS: circular shift by `bound` before the spline (forward) / after it (inverse)
     int use_bulk;  // host-side verdict: alignment rules for cp.async.bulk hold for full tiles
     int iters;     // Gaussianization inverse: bisection steps
+    sosp::Const sosp;  // SOSP: shape, bisection and pre-scaled quadrature
 };
+
+// SOSP pair: the default shape works on a register copy of its 16 parameters (four 16-byte loads:
+// P = 16 puts every pair on the same banks, a 4-way rather than a 16-way conflict)
+template <int KT, bool INVERSE, bool FAST>
+__device__ __forceinline__ float sosp_pair(const float* pp, const sosp::Const& c, float xv, float& lj) {
+    auto run = [&](const float* ap) {
+        if constexpr (INVERSE) {
+            return sosp::inverse<KT>(ap, c, xv);
+        } else {
+            float gx;
+            const float yv = sosp::forward<KT>(ap, c, xv, gx);
+            lj = zlog<FAST>(gx);
+            return yv;
+        }
+    };
+    if constexpr (KT > 0) {
+        float ar[sosp::kDefP];
+#pragma unroll
+        for (int q = 0; q < sosp::kDefP / 4; ++q) {
+            const float4 v = reinterpret_cast<const float4*>(pp)[q];
+            ar[4 * q] = v.x; ar[4 * q + 1] = v.y; ar[4 * q + 2] = v.z; ar[4 * q + 3] = v.w;
+        }
+        return run(ar);
+    } else {
+        return run(pp);
+    }
+}
 
 // UNI: ZK_UNI_*; KT: compile-time bins (0 = runtime K); INVERSE; FAST math
 template <int UNI, int KT, bool INVERSE, bool FAST>
@@ -116,6 +146,8 @@ __global__ void __launch_bounds__(kUniThreads) uni_kernel(const UniParams a) {
                 } else {
                     yv = gauss_inverse_eval<KT, FAST>(pp, a.K, xv, a.bound, a.iters);
                 }
+            } else if constexpr (UNI == ZK_UNI_SOSP) {
+                yv = sosp_pair<KT, INVERSE, FAST>(pp, a.sosp, xv, lj);
             } else {  // affine, transforms.py:435-446: phi = (shift, unconstrained log-scale)
                 const float shift = pp[0];
                 const float ls = softclip<FAST>(pp[1], a.ad);
@@ -186,6 +218,11 @@ zk_status launch_uni_dir(const UniParams& p, int uni, bool fast, int grid, size_
             default: return launch_uni_t<ZK_UNI_GAUSS, 0, INVERSE>(p, fast, grid, smem, st);
         }
     }
+    if (uni == ZK_UNI_SOSP) {
+        if (p.sosp.K == sosp::kDefK && p.sosp.L == sosp::kDefL)
+            return launch_uni_t<ZK_UNI_SOSP, sosp::kDefK, INVERSE>(p, fast, grid, smem, st);
+        return launch_uni_t<ZK_UNI_SOSP, 0, INVERSE>(p, fast, grid, smem, st);
+    }
     switch (p.K) {
         case 4: return launch_uni_t<ZK_UNI_RQS, 4, INVERSE>(p, fast, grid, smem, st);
         case 8: return launch_uni_t<ZK_UNI_RQS, 8, INVERSE>(p, fast, grid, smem, st);
@@ -200,18 +237,22 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     ZK_REQUIRE(a.B >= 0 && a.D > 0, "univariate: bad shape B=%lld D=%d", (long long)a.B, a.D);
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate: null input");
-    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS,
+    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS ||
+                   a.univariate == ZK_UNI_SOSP,
                "univariate: unknown kind %d", a.univariate);
-    int P = 2;
     if (a.univariate == ZK_UNI_RQS) {
         ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "rqs: bins must be in [1, 1024], got %d", a.K);
-        P = 3 * a.K - 1;
     } else if (a.univariate == ZK_UNI_GAUSS) {
         ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "gaussianization: components must be in [1, 1024], got %d", a.K);
         ZK_REQUIRE(a.bound > 0.f, "gaussianization: bound must be positive");
         if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "gaussianization: bisection steps must be in [1, 64], got %d", a.iters);
-        P = 2 * a.K;
+    } else if (a.univariate == ZK_UNI_SOSP) {
+        ZK_REQUIRE(sosp_shape_ok(a.K, a.degree), "sosp: polynomials %d / degree %d out of range (degree <= 15, K (degree + 1) + 1 <= 1024)",
+                   a.K, a.degree);
+        ZK_REQUIRE(a.bound > 0.f, "sosp: bound must be positive");
+        if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "sosp: bisection steps must be in [1, 64], got %d", a.iters);
     }
+    const int P = uni_param_count(a.univariate, a.K, a.degree);
     ZK_REQUIRE(a.phi_ld == 0 || a.phi_ld >= (int64_t)a.D * P, "univariate: phi_ld too small");
     ZK_REQUIRE(a.slope > 0.f && a.slope < 1.f, "univariate: slope must be in (0, 1)");
     if (a.inverse) ZK_REQUIRE(a.y != nullptr, "univariate inverse: null output");
@@ -224,6 +265,7 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     p.dim_map = a.dim_map; p.B = a.B; p.D = a.D; p.K = a.K; p.P = P; p.bound = a.bound;
     p.circ = (a.circular && a.univariate == ZK_UNI_RQS) ? 1 : 0;
     p.iters = a.iters;
+    if (a.univariate == ZK_UNI_SOSP) p.sosp = sosp::make_const(a.K, a.degree, a.bound, a.slope, a.iters);
     const float absL = fabsf(logf(a.slope));
     p.aw = 2.f / absL;
     p.ad = 1.f / absL;

@@ -24,9 +24,10 @@ struct UniArgs {
     const int* dim_map = nullptr;  // (D) device: pair d lives in column dim_map[d] of x / y (coupling)
     int64_t B = 0;
     int D = 0;      // number of transformed dims (pairs per sample)
-    int K = 0;      // bins (RQS) / mixture components (Gaussianization)
+    int K = 0;      // bins (RQS) / mixture components (Gaussianization) / polynomials (SOSP)
+    int degree = 0; // SOSP: polynomial degree L
     float bound = 5.f;
-    int iters = 0;  // Gaussianization inverse: bisection steps on [-bound, bound]
+    int iters = 0;  // Gaussianization / SOSP inverse: bisection steps on [-bound, bound]
     float slope = 1e-3f;
     bool circular = false;  // RQS only: CircularShiftTransform(bound) in front (forward) / behind (inverse)
     bool fast_math = true;  // MUFU rcp/ex2/lg2 fast path (default) vs IEEE div + expf/logf

@@ -19,6 +19,7 @@ from ..transforms import (
     GaussianizationTransform,
     MonotonicAffineTransform,
     MonotonicRQSTransform,
+    ShiftedSOSPTransform,
     bisection_steps,
 )
 
@@ -68,9 +69,22 @@ def resolve_univariate(univariate: Callable, shapes: Sequence[Size]) -> dict:
         K = shapes[0][0]
         bound, eps = float(kwargs.get("bound", 10.0)), float(kwargs.get("eps", 1e-6))
         return dict(kind=E.ZK_UNI_GAUSS, bins=K, bound=bound, slope=1e-3, total=2 * K, iterations=bisection_steps(bound, eps))
+    if f is ShiftedSOSPTransform:  # flows/polynomial.py:23-28, 66-72: SOSPolynomialTransform's bound / eps defaults
+        if len(shapes) != 2 or len(shapes[0]) != 2 or shapes[1] != ():
+            raise ValueError(f"ShiftedSOSPTransform expects shapes [(K, L+1), ()], got {shapes}")
+        extra = set(kwargs) - {"slope"}
+        if extra:
+            raise NotImplementedError(f"zuko_b200: unsupported ShiftedSOSPTransform arguments {sorted(extra)}")
+        K, n = shapes[0]
+        if K < 1 or not 1 <= n <= 16 or K * n + 1 > 1024:
+            raise NotImplementedError(f"zuko_b200: ShiftedSOSPTransform with {K} polynomials of degree {n - 1} "
+                                      "(the engine takes degree <= 15 and K (degree + 1) + 1 <= 1024)")  # fmt: skip
+        return dict(kind=E.ZK_UNI_SOSP, bins=K, degree=n - 1, bound=10.0, slope=float(kwargs.get("slope", 1e-3)),
+                    total=K * n + 1, iterations=bisection_steps(10.0, 1e-6))  # fmt: skip
     raise NotImplementedError(
         f"zuko_b200: univariate transformation {getattr(f, '__name__', f)!r} is not implemented by the engine "
-        "(supported: MonotonicAffineTransform, MonotonicRQSTransform, CircularRQSTransform, GaussianizationTransform)"
+        "(supported: MonotonicAffineTransform, MonotonicRQSTransform, CircularRQSTransform, GaussianizationTransform, "
+        "ShiftedSOSPTransform)"
     )
 
 
@@ -79,6 +93,13 @@ def refuse_elementwise_only(uni: dict, layer: str) -> None:
     element-wise layers only (flows/gaussianization.py:97-155)."""
     if uni["kind"] == E.ZK_UNI_GAUSS:
         raise NotImplementedError(f"zuko_b200: GaussianizationTransform is supported in element-wise layers only, not in {layer}")
+
+
+def refuse_autoregressive_only(uni: dict, layer: str) -> None:
+    """The sum-of-squares polynomial bijector runs in masked autoregressive layers only
+    (flows/polynomial.py:31-76)."""
+    if uni["kind"] == E.ZK_UNI_SOSP:
+        raise NotImplementedError(f"zuko_b200: ShiftedSOSPTransform is supported in autoregressive layers only, not in {layer}")
 
 
 class OwnedLayer:
@@ -216,9 +237,11 @@ class PackedLayerMixin:
         u = self._uni
         return E.LayerDesc(kind=kind, features=self.features, context=self.context, univariate=u["kind"],
                            bins=u["bins"], bound=u["bound"], slope=u["slope"], passes=getattr(self, "passes", 0),
-                           iterations=u.get("iterations", 0))  # fmt: skip
+                           iterations=u.get("iterations", 0), degree=u.get("degree", 0))  # fmt: skip
 
     def _describe_base(self) -> str:
+        if self._uni["kind"] == E.ZK_UNI_SOSP:
+            return "ShiftedSOSPTransform(polynomials=%d, degree=%d)" % (self._uni["bins"], self._uni["degree"])
         if self._uni["kind"] == E.ZK_UNI_GAUSS:
             return "GaussianizationTransform(components=%d)" % self._uni["bins"]
         if self._uni["kind"] == E.ZK_UNI_CRQS:

@@ -16,7 +16,7 @@ from ..distributions import DiagNormal
 from ..lazy import Flow, LazyTransform, UnconditionalDistribution
 from ..nn import MLP
 from ..transforms import CouplingTransform, MonotonicAffineTransform
-from ._packed import PackedLayerMixin, refuse_elementwise_only, resolve_univariate, total_of
+from ._packed import PackedLayerMixin, refuse_autoregressive_only, refuse_elementwise_only, resolve_univariate, total_of
 from .elementwise import ElementWiseTransform
 
 
@@ -45,6 +45,7 @@ class GeneralCouplingTransform(PackedLayerMixin, LazyTransform):
         self.total = total_of(shapes)
         self._uni = resolve_univariate(univariate, shapes)
         refuse_elementwise_only(self._uni, "GeneralCouplingTransform")
+        refuse_autoregressive_only(self._uni, "GeneralCouplingTransform")
         self.features, self.context = features, context
         mask = torch.arange(features) % 2 == 1 if mask is None else torch.as_tensor(mask, dtype=bool)
         assert mask.ndim == 1, "'mask' should be a vector."

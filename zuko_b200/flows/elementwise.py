@@ -16,7 +16,7 @@ from .. import _engine as E
 from ..lazy import LazyTransform
 from ..nn import MLP
 from ..transforms import DependentTransform, MonotonicAffineTransform
-from ._packed import PackedLayerMixin, resolve_univariate, total_of
+from ._packed import PackedLayerMixin, refuse_autoregressive_only, resolve_univariate, total_of
 
 
 class ElementWiseTransform(PackedLayerMixin, LazyTransform):
@@ -36,6 +36,7 @@ class ElementWiseTransform(PackedLayerMixin, LazyTransform):
         self.univariate, self.shapes = univariate, shapes
         self.total = total_of(shapes)
         self._uni = resolve_univariate(univariate, shapes)
+        refuse_autoregressive_only(self._uni, "ElementWiseTransform")
         self.features, self.context = features, context
         if context > 0:
             self.hyper = MLP(context, features * self.total, **kwargs)

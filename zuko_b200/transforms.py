@@ -7,7 +7,8 @@ C ABI of the H100 engine; no torch arithmetic runs here.
 
 * univariate bijectors built from explicit parameters:
   ``MonotonicRQSTransform`` (transforms.py:449-567), ``MonotonicAffineTransform``
-  (:412-446), ``GaussianizationTransform`` (:834-875), ``SoftclipTransform`` (:286-316);
+  (:412-446), ``GaussianizationTransform`` (:834-875), ``SOSPolynomialTransform`` (:931-963,
+  with ``ShiftedSOSPTransform`` of zuko/flows/polynomial.py:23-28), ``SoftclipTransform`` (:286-316);
 * linear maps: ``PermutationTransform`` (:1182-1214), ``RotationTransform`` (:1217-1244);
 * packed conditional layers produced by the lazy modules in ``zuko_b200.flows``:
   ``AutoregressiveTransform`` (:966-1007), ``CouplingTransform`` (:1010-1073),
@@ -30,6 +31,8 @@ __all__ = [
     "MonotonicRQSTransform",
     "PermutationTransform",
     "RotationTransform",
+    "SOSPolynomialTransform",
+    "ShiftedSOSPTransform",
     "SoftclipTransform",
 ]
 
@@ -153,6 +156,9 @@ def _uni_forward(kind: int, K: int, bound: float, slope: float, x2: Tensor, phi:
             E.check(L.zk_rqs_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, K, bound, slope, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
         elif kind == E.ZK_UNI_GAUSS:
             E.check(L.zk_gaussianization_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, K, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
+        elif kind == E.ZK_UNI_SOSP:
+            (K, deg) = K
+            E.check(L.zk_sosp_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, K, deg, bound, slope, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
         elif kind == E.ZK_UNI_AFFINE:
             E.check(L.zk_affine_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, slope, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
         else:
@@ -162,8 +168,9 @@ def _uni_forward(kind: int, K: int, bound: float, slope: float, x2: Tensor, phi:
 
 class _UniFunction(torch.autograd.Function):
     """Autograd seam of the explicit-parameter bijectors: backward = ``zk_rqs_backward`` /
-    ``zk_affine_backward`` / ``zk_gaussianization_backward`` / ``zk_softclip_backward`` (reverse mode
-    of transforms.py:469-567, 426-446, 834-875, 299-316)."""
+    ``zk_affine_backward`` / ``zk_gaussianization_backward`` / ``zk_sosp_backward`` / ``zk_softclip_backward``
+    (reverse mode of transforms.py:469-567, 426-446, 834-875, 878-963, 299-316).  ``K`` is the pair
+    ``(polynomials, degree)`` for the sum-of-squares polynomial bijector."""
 
     @staticmethod
     def forward(ctx, kind, K, bound, slope, ld, x2, phi):  # noqa: ANN001
@@ -201,6 +208,8 @@ class _UniFunction(torch.autograd.Function):
                 E.check(L.zk_rqs_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, K, bound, slope, *args))
             elif kind == E.ZK_UNI_GAUSS:
                 E.check(L.zk_gaussianization_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, K, *args))
+            elif kind == E.ZK_UNI_SOSP:
+                E.check(L.zk_sosp_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, *K, bound, slope, *args))
             else:
                 E.check(L.zk_affine_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, slope, *args))
         return None, None, None, None, None, gx, gphi
@@ -329,6 +338,58 @@ class GaussianizationTransform(EngineTransform):
             E.check(E.lib().zk_gaussianization_inverse(y2.data_ptr(), 1, phi.data_ptr(), ld, y2.shape[0], 1, self.components,
                                                        self.bound, self.iterations, x.data_ptr(), 1, E.stream_ptr(y2.device)))  # fmt: skip
         return x.reshape(shape)
+
+
+class SOSPolynomialTransform(EngineTransform):
+    """Sum-of-squares polynomial bijector ``f(x) = int_0^x (1/K) sum_k (1 + sum_j a_kj (u / bound)^j)^2 du + slope x``
+    with coefficients ``a`` of shape ``(*, K, L + 1)`` (zuko/transforms.py:931-963).  ``zk_sosp_forward`` evaluates
+    the reference's ``L + 1``-node Gauss-Legendre quadrature and ``ladj = log g(x)``; the inverse runs the
+    reference's ``ceil(log2(2 bound / eps))`` bisection steps on ``[-bound, bound]`` (transforms.py:609-617) in
+    ``zk_sosp_inverse``.  Gradients: ``zk_sosp_backward``."""
+
+    domain = constraints.real
+    codomain = constraints.real
+
+    def __init__(self, a: Tensor, slope: float = 1e-3, bound: float = 10.0, eps: float = 1e-6) -> None:
+        super().__init__()
+        self._setup(a, a.new_zeros(()), slope, bound, eps)
+
+    def _setup(self, a: Tensor, constant: Tensor, slope: float, bound: float, eps: float) -> None:
+        self.polynomials, n = a.shape[-2:]
+        self.degree = n - 1
+        batch = torch.broadcast_shapes(a.shape[:-2], constant.shape)
+        a = a.expand(*batch, self.polynomials, n).flatten(-2)
+        # (*, K (L + 1) + 1): the layout of MaskedAutoregressiveTransform's split for shapes [(K, L + 1), ()]
+        self.phi = torch.cat((a, constant.expand(batch)[..., None].to(a.dtype)), dim=-1)
+        self.slope, self.bound, self.eps = float(slope), float(bound), float(eps)
+        self.iterations = bisection_steps(self.bound, self.eps)
+
+    def __repr__(self) -> str:
+        return f"{type(self).__name__}(polynomials={self.polynomials}, degree={self.degree})"
+
+    def call_and_ladj(self, x: Tensor) -> tuple[Tensor, Tensor]:
+        x2, phi, ld, shape = _elementwise(self.phi, x, self.phi.shape[-1])
+        y, ladj = _uni_call(E.ZK_UNI_SOSP, (self.polynomials, self.degree), self.bound, self.slope, x2, phi, ld)
+        return y.reshape(shape), ladj.reshape(shape)
+
+    def _inverse(self, y: Tensor) -> Tensor:
+        _no_grad_inverse(y, self.phi)
+        y2, phi, ld, shape = _elementwise(self.phi.detach(), y.detach(), self.phi.shape[-1])
+        x = torch.empty_like(y2)
+        with torch.cuda.device(y2.device):
+            E.check(E.lib().zk_sosp_inverse(y2.data_ptr(), 1, phi.data_ptr(), ld, y2.shape[0], 1, self.polynomials, self.degree,
+                                            self.bound, self.slope, self.iterations, x.data_ptr(), 1, E.stream_ptr(y2.device)))  # fmt: skip
+        return x.reshape(shape)
+
+
+def ShiftedSOSPTransform(a: Tensor, constant: Tensor, slope: float = 1e-3) -> Transform:
+    """``SOSPolynomialTransform(a, slope)`` followed by ``AdditiveTransform(constant)`` (zuko/flows/polynomial.py:23-28)
+    as ONE engine transform: the constant is the last parameter of each pair and the kernels add it (forward) or
+    subtract it before the bisection (inverse)."""
+    t = SOSPolynomialTransform.__new__(SOSPolynomialTransform)
+    EngineTransform.__init__(t)
+    t._setup(a, constant, slope, 10.0, 1e-6)
+    return t
 
 
 class SoftclipTransform(EngineTransform):
