@@ -248,6 +248,11 @@ int zk_layer_fused_info(const zk_layer* layer, double* out);
 /* Rows per tile of the fused layer kernel for this layer, chosen from its shape: 128 (two consumer warpgroups
  * share every streamed weight tile), 64, or 0 when the layer does not run as the fused kernel.  Read-only. */
 int zk_layer_fused_tile_rows(const zk_layer* layer);
+/* Launch geometry of the layer's dimension-sequential inverse kernel, as its next launch would choose it
+ * (the ZK_INV_GEOM=TxR override included): threads per CTA, samples per thread and dynamic shared memory
+ * bytes.  Returns 1 and fills the non-NULL outputs when the layer's inverse runs as that kernel (with the
+ * fused kernels enabled, zk_set_fused_layers), 0 when it runs the `passes` sweeps.  Read-only. */
+int zk_layer_inverse_geometry(const zk_layer* layer, int* threads, int* samples_per_thread, size_t* smem);
 /* 1 when the layer's inverse runs as the dimension-sequential kernel (one launch, emits the ladj): the
  * precondition for using it as an inverted member of a zk_flow_desc. */
 int zk_layer_sequential_inverse(const zk_layer* layer);

@@ -488,6 +488,17 @@ int zk_layer_sequential_inverse(const zk_layer* l) {
     return (l && l->kind == ZK_LAYER_AUTOREGRESSIVE && (l->inv != nullptr || l->inv_dirty)) ? 1 : 0;
 }
 
+int zk_layer_inverse_geometry(const zk_layer* l, int* threads, int* samples_per_thread, size_t* smem) {
+    if (!l || l->kind != ZK_LAYER_AUTOREGRESSIVE || !l->inv) return 0;
+    int T = 0, R = 0;
+    size_t bytes = 0;
+    if (!ar_inverse_geometry(l->inv, &T, &R, &bytes)) return 0;
+    if (threads) *threads = T;
+    if (samples_per_thread) *samples_per_thread = R;
+    if (smem) *smem = bytes;
+    return 1;
+}
+
 int zk_layer_fused_info(const zk_layer* l, double* out) {
     if (!l || !out) return -1;
     out[0] = out[1] = out[2] = out[3] = 0.0;

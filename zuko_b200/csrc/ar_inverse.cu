@@ -556,6 +556,10 @@ bool ar_inverse_threads(const ArInvPack* pk, int* threads, size_t* smem) {
     return inv_geometry(pk, threads, &R, smem);
 }
 
+bool ar_inverse_geometry(const ArInvPack* pk, int* threads, int* per_thread, size_t* smem) {
+    return inv_geometry(pk, threads, per_thread, smem);
+}
+
 zk_status launch_ar_inverse(const ArInvPack* pk, const ArInvArgs& a, cudaStream_t st) {
     if (a.B == 0) return ZK_OK;
     int T = 0, R = 0;

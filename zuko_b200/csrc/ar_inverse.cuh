@@ -15,6 +15,9 @@ zk_status ar_inverse_pack(const zk_mlp* m, const uint8_t* const* mask_dev, const
                           int univariate, int bins, int degree, int passes, ArInvPack** out);
 void ar_inverse_free(ArInvPack* pk);
 bool ar_inverse_threads(const ArInvPack* pk, int* threads, size_t* smem);
+// the launch geometry launch_ar_inverse uses (ZK_INV_GEOM honoured): threads per CTA, samples per
+// thread, dynamic shared memory; false when the state does not fit
+bool ar_inverse_geometry(const ArInvPack* pk, int* threads, int* per_thread, size_t* smem);
 
 struct ArInvArgs {
     const float* y = nullptr; int64_t ldy = 0;  // the layer's output (input of the inverse)
