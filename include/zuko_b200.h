@@ -248,6 +248,11 @@ int zk_layer_fused_info(const zk_layer* layer, double* out);
 /* Rows per tile of the fused layer kernel for this layer, chosen from its shape: 128 (two consumer warpgroups
  * share every streamed weight tile), 64, or 0 when the layer does not run as the fused kernel.  Read-only. */
 int zk_layer_fused_tile_rows(const zk_layer* layer);
+/* The fused layer kernel's plan for this layer, as its next launch would choose it: returns the rows per tile (the
+ * value of zk_layer_fused_tile_rows) and, when it is not 0, fills the non-NULL outputs with the number of 16 KB
+ * weight-ring slots (64-row tiles: both consumer warpgroups' rings together) and the dynamic shared memory bytes.
+ * Read-only. */
+int zk_layer_fused_plan(const zk_layer* layer, int* ring_slots, size_t* smem);
 /* Launch geometry of the layer's dimension-sequential inverse kernel, as its next launch would choose it
  * (the ZK_INV_GEOM=TxR override included): threads per CTA, samples per thread and dynamic shared memory
  * bytes.  Returns 1 and fills the non-NULL outputs when the layer's inverse runs as that kernel (with the

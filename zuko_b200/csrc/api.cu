@@ -521,6 +521,11 @@ int zk_layer_fused_tile_rows(const zk_layer* l) {
     return fused_tile_rows(l->hyper, l->uni, l->K, l->D, l->C);
 }
 
+int zk_layer_fused_plan(const zk_layer* l, int* ring_slots, size_t* smem) {
+    if (!l || l->kind != ZK_LAYER_AUTOREGRESSIVE || !l->hyper || l->circ) return 0;
+    return fused_layer_plan(l->hyper, l->uni, l->K, l->D, l->C, ring_slots, smem);
+}
+
 size_t zk_layer_workspace_bytes(const zk_layer* l, int64_t B) {
     if (!l || B <= 0) return 0;
     switch (l->kind) {

@@ -508,9 +508,16 @@ static int fused_kba(const zk_mlp* m) {
     return std::max(((const TcPack*)m->tc)->layers[0].Kp / FK, m->dims[1] / FK);
 }
 
-int fused_tile_rows(const zk_mlp* m, int univariate, int bins, int D, int C) {
+int fused_layer_plan(const zk_mlp* m, int univariate, int bins, int D, int C, int* ring_slots, size_t* smem) {
     if (!fused_layer_supported(m, univariate, bins, D, C)) return 0;
-    return fused_plan(fused_kba(m), univariate, bins).rows;
+    const FusedPlan plan = fused_plan(fused_kba(m), univariate, bins);
+    if (ring_slots) *ring_slots = plan.n_stages;
+    if (smem) *smem = plan.smem;
+    return plan.rows;
+}
+
+int fused_tile_rows(const zk_mlp* m, int univariate, int bins, int D, int C) {
+    return fused_layer_plan(m, univariate, bins, D, C, nullptr, nullptr);
 }
 
 namespace {

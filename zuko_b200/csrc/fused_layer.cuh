@@ -29,6 +29,9 @@ bool fused_layer_supported(const zk_mlp* m, int univariate, int bins, int D, int
 int fused_layer_kind(const zk_mlp* m, int univariate, int bins, int D, int C);
 // rows per tile of the fused layer kernel for this layer (64 or 128, from the shape); 0 when it does not run fused
 int fused_tile_rows(const zk_mlp* m, int univariate, int bins, int D, int C);
+// the same, with the plan launch_fused_layer uses: W ring slots (64-row tiles: both rings together) and dynamic
+// shared memory bytes (outputs may be null; untouched when the layer does not run fused)
+int fused_layer_plan(const zk_mlp* m, int univariate, int bins, int D, int C, int* ring_slots, size_t* smem);
 // Builds the fused kernel's weight pack for this conditioner (degree-sorted hidden units, zero-tile
 // map); `mask_dev` are the DEVICE mask pointers of zk_mlp_desc (may be null = dense).  No-op when
 // the shape is not supported by the fused kernel.
