@@ -55,6 +55,10 @@ typedef void* zk_stream; /* cudaStream_t */
                            zuko/flows/polynomial.py:23-28, transforms.py:878-963; phi = (a[K][L+1] row-major, constant),
                            P = K (L + 1) + 1 (K = `bins`, L = `degree`); inverse by bisection on [-bound, bound];
                            autoregressive layers only */
+#define ZK_UNI_BERNSTEIN 6 /* BoundedBernsteinTransform, zuko/transforms.py:640-831 (BPF, flows/polynomial.py:79-117);
+                              phi = u[degree + 1] (unconstrained, softmax-constrained coefficient differences),
+                              order M = degree + 5 <= 64; bound B = `bound`, eps = 1e-6; inverse by the two linear
+                              branches beyond [-B, B] and bisection on [-B, B] inside; autoregressive layers only */
 /* base distribution of a flow */
 #define ZK_BASE_DIAG_NORMAL 0 /* DiagNormal(loc, scale)    zuko/distributions.py:337-363 */
 #define ZK_BASE_BOX_UNIFORM 1 /* BoxUniform(lower, upper)  zuko/distributions.py:366-396; base_loc = lower, base_scale = upper */
@@ -136,6 +140,16 @@ zk_status zk_sosp_forward(const float* x, int64_t ldx, const float* phi, int64_t
 zk_status zk_sosp_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B, int D,
                           int K, int degree, float bound, float slope, int iterations, float* x, int64_t ldx,
                           zk_stream stream);
+/* BoundedBernsteinTransform(u, bound, eps) — transforms.py:640-831; phi = u[degree + 1] per pair, 0 <= degree <= 59,
+ * bound > 0, 0 < eps < 1/2.  Forward: t = (x + B) / 2B; y = sum_i theta_i b_{i,M}(t) for eps < t < 1 - eps, else
+ * the linear branches 2B (t - eps) - B and 2B (t - 1 + eps) + B (so x -+ 2B eps outside [-B, B]), and ladj =
+ * log f'(x) (0 in the linear branches).  Inverse: the linear branches exactly for y <= -B and y >= B, else
+ * ceil(log2(2 B / eps)) bisection steps on [-B, B] (utils.py:159-183). */
+zk_status zk_bernstein_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
+                               int degree, float bound, float eps, float* y, int64_t ldy, float* ladj,
+                               int accumulate, zk_stream stream);
+zk_status zk_bernstein_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B, int D,
+                               int degree, float bound, float eps, float* x, int64_t ldx, zk_stream stream);
 /* SoftclipTransform(bound)                       — transforms.py:299-316 */
 zk_status zk_softclip_forward(const float* x, int64_t ldx, int64_t B, int D, float bound, float* y,
                               int64_t ldy, float* ladj, int accumulate, zk_stream stream);
@@ -211,7 +225,8 @@ typedef struct {
     int context;    /* C (0 = unconditional) */
     int univariate; /* ZK_UNI_* (autoregressive / coupling / elementwise) */
     int bins;       /* K for ZK_UNI_RQS, mixture components K for ZK_UNI_GAUSS, polynomials K for ZK_UNI_SOSP */
-    float bound;    /* spline bound B (5.0), softclip bound or the bisection bound of ZK_UNI_GAUSS / ZK_UNI_SOSP (10.0) */
+    float bound;    /* spline bound B (5.0), softclip bound, the bisection bound of ZK_UNI_GAUSS / ZK_UNI_SOSP (10.0)
+                       or the Bernstein bound B of ZK_UNI_BERNSTEIN (5.0) */
     float slope;    /* minimum slope (1e-3) */
     int passes;     /* autoregressive: number of inverse sweeps (transforms.py:994-1000) */
     const int64_t* order;         /* host (D): autoregressive order classes (MaskedAutoregressiveTransform.order,
@@ -220,8 +235,9 @@ typedef struct {
     const zk_mlp_desc* hyper;     /* conditioner; NULL for parameter-free / shared-table layers */
     const float* phi;             /* DEVICE (D, P) shared table: elementwise without context */
     const float* rotation;        /* DEVICE (D, D) R for ZK_LAYER_ROTATION */
-    int iterations;               /* ZK_UNI_GAUSS / ZK_UNI_SOSP: bisection steps of the inverse, ceil(log2(2 bound / eps)) (>= 1) */
-    int degree;                   /* ZK_UNI_SOSP: polynomial degree L (0 .. 15) */
+    int iterations;               /* ZK_UNI_GAUSS / ZK_UNI_SOSP / ZK_UNI_BERNSTEIN: bisection steps of the inverse,
+                                     ceil(log2(2 bound / eps)) (>= 1; eps = 1e-6) */
+    int degree;                   /* ZK_UNI_SOSP: polynomial degree L (0 .. 15); ZK_UNI_BERNSTEIN: BPF degree (0 .. 59) */
 } zk_layer_desc;
 
 zk_status zk_layer_create(const zk_layer_desc* desc, zk_layer** out);
@@ -373,6 +389,11 @@ zk_status zk_sosp_backward(const float* x, int64_t ldx, const float* phi, int64_
                            int K, int degree, float bound, float slope, const float* grad_y, int64_t ldgy,
                            const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi, void* workspace,
                            size_t workspace_bytes, zk_stream stream);
+/* same for BoundedBernsteinTransform (transforms.py:640-831), P = degree + 1 */
+zk_status zk_bernstein_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
+                                int degree, float bound, float eps, const float* grad_y, int64_t ldgy,
+                                const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi, void* workspace,
+                                size_t workspace_bytes, zk_stream stream);
 /* SoftclipTransform (transforms.py:299-316) */
 zk_status zk_softclip_backward(const float* x, int64_t ldx, int64_t B, int D, float bound,
                                const float* grad_y, int64_t ldgy, const float* grad_ladj,
@@ -449,7 +470,8 @@ int zk_set_tc_backward(int on);
 /* Transcendental arithmetic of the bijector kernels: 1 (default) = MUFU rcp / ex2 / lg2
  * approximations, 0 = IEEE division + expf / logf (erf / erfc / erfcinv of the Gaussianization
  * bijector are IEEE-library calls in both settings; the sum-of-squares polynomial bijector uses the
- * approximation only for the log of its ladj).  Process-wide; returns the previous
+ * approximation only for the log of its ladj, the bounded Bernstein bijector only for the log of its
+ * ladj).  Process-wide; returns the previous
  * value.  Both settings meet the 1e-5 parity bar on the BASELINE configs (tests/). */
 int zk_set_fast_math(int on);
 /* 1 (default): an autoregressive layer whose conditioner fits the fused kernel (hidden widths

@@ -21,7 +21,7 @@ LIB_PATH = Path(__file__).resolve().parent / "lib" / "libzuko_b200.so"
 
 # status codes (include/zuko_b200.h)
 ZK_OK, ZK_EINVAL, ZK_EUNSUPPORTED, ZK_ECUDA, ZK_ENOMEM = range(5)
-ZK_UNI_AFFINE, ZK_UNI_RQS, ZK_UNI_CRQS, ZK_UNI_GAUSS, ZK_UNI_SOSP = 1, 2, 3, 4, 5
+ZK_UNI_AFFINE, ZK_UNI_RQS, ZK_UNI_CRQS, ZK_UNI_GAUSS, ZK_UNI_SOSP, ZK_UNI_BERNSTEIN = 1, 2, 3, 4, 5, 6
 ZK_BASE_DIAG_NORMAL, ZK_BASE_BOX_UNIFORM = 0, 1
 (
     ZK_LAYER_AUTOREGRESSIVE,
@@ -117,6 +117,8 @@ _SIGNATURES = {
     "zk_gaussianization_inverse": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_float, c_int, _P, c_int64, _P]),
     "zk_sosp_forward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_int, c_float, c_float, _P, c_int64, _P, c_int, _P]),
     "zk_sosp_inverse": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_int, c_float, c_float, c_int, _P, c_int64, _P]),
+    "zk_bernstein_forward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_float, c_float, _P, c_int64, _P, c_int, _P]),
+    "zk_bernstein_inverse": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_float, c_float, _P, c_int64, _P]),
     "zk_softclip_forward": (c_int, [_P, c_int64, c_int64, c_int, c_float, _P, c_int64, _P, c_int, _P]),
     "zk_softclip_inverse": (c_int, [_P, c_int64, c_int64, c_int, c_float, _P, c_int64, _P]),
     "zk_permute": (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, _P]),
@@ -159,6 +161,7 @@ _SIGNATURES = {
     "zk_affine_backward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_float, _P, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),
     "zk_gaussianization_backward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, _P, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),
     "zk_sosp_backward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_int, c_float, c_float, _P, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),
+    "zk_bernstein_backward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_float, c_float, _P, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),
     "zk_softclip_backward": (c_int, [_P, c_int64, c_int64, c_int, c_float, _P, c_int64, _P, _P, c_int64, _P]),
     "zk_layer_backward_workspace_bytes": (c_size_t, [_P, c_int64]),
     "zk_layer_backward": (c_int, [_P, _P, c_int64, _P, c_int64, c_int64, _P, c_int64, _P, _P, c_int64, _P, c_int64, POINTER(LayerGrads), _P, c_size_t, _P]),

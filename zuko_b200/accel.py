@@ -53,6 +53,7 @@ _ENGINE_CALLABLES = {
     "SoftclipTransform": _T.SoftclipTransform,
     "ShiftedSOSPTransform": _T.ShiftedSOSPTransform,
     "SOSPolynomialTransform": _T.SOSPolynomialTransform,
+    "BoundedBernsteinTransform": _T.BoundedBernsteinTransform,
     "PermutationTransform": _T.PermutationTransform,
     "RotationTransform": _T.RotationTransform,
 }

@@ -150,6 +150,32 @@ zk_status zk_sosp_inverse(const float* y, int64_t ldy, const float* phi, int64_t
     return launch_univariate(a, (cudaStream_t)stream);
 }
 
+// ceil(log2(2 bound / eps)) (MonotonicTransform._inverse, transforms.py:609-617); 0 when out of range
+static int bisection_steps(float bound, float eps) {
+    if (!(bound > 0.f) || !(eps > 0.f)) return 0;
+    const double n = ceil(log2(2.0 * (double)bound / (double)eps));
+    return (n >= 1.0 && n <= 64.0) ? (int)n : 0;
+}
+
+zk_status zk_bernstein_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
+                               int degree, float bound, float eps, float* y, int64_t ldy, float* ladj,
+                               int accumulate, zk_stream stream) {
+    UniArgs a;
+    a.univariate = ZK_UNI_BERNSTEIN; a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = phi_ld; a.B = B; a.D = D;
+    a.degree = degree; a.bound = bound; a.eps = eps; a.y = y; a.ldy = ldy; a.ladj = ladj;
+    a.accumulate = accumulate; a.fast_math = g_fast_math.load() != 0;
+    return launch_univariate(a, (cudaStream_t)stream);
+}
+
+zk_status zk_bernstein_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B, int D,
+                               int degree, float bound, float eps, float* x, int64_t ldx, zk_stream stream) {
+    UniArgs a;
+    a.univariate = ZK_UNI_BERNSTEIN; a.inverse = true; a.x = y; a.ldx = ldy; a.phi = phi; a.phi_ld = phi_ld;
+    a.B = B; a.D = D; a.degree = degree; a.bound = bound; a.eps = eps; a.iters = bisection_steps(bound, eps);
+    a.y = x; a.ldy = ldx; a.fast_math = g_fast_math.load() != 0;
+    return launch_univariate(a, (cudaStream_t)stream);
+}
+
 zk_status zk_softclip_forward(const float* x, int64_t ldx, int64_t B, int D, float bound, float* y,
                               int64_t ldy, float* ladj, int accumulate, zk_stream stream) {
     return launch_softclip(x, ldx, B, D, bound, false, y, ldy, ladj, accumulate, (cudaStream_t)stream);
@@ -350,7 +376,8 @@ static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
     const bool has_uni = (l->kind == ZK_LAYER_AUTOREGRESSIVE || l->kind == ZK_LAYER_COUPLING ||
                           l->kind == ZK_LAYER_ELEMENTWISE);
     if (has_uni) {
-        ZK_REQUIRE(l->uni == ZK_UNI_AFFINE || l->uni == ZK_UNI_RQS || l->uni == ZK_UNI_GAUSS || l->uni == ZK_UNI_SOSP,
+        ZK_REQUIRE(l->uni == ZK_UNI_AFFINE || l->uni == ZK_UNI_RQS || l->uni == ZK_UNI_GAUSS || l->uni == ZK_UNI_SOSP ||
+                       l->uni == ZK_UNI_BERNSTEIN,
                    "layer_create: univariate=%d", d->univariate);
         if (l->uni == ZK_UNI_GAUSS) {  // the bisection inverse is element-wise only (flows/gaussianization.py:97-155)
             if (l->kind != ZK_LAYER_ELEMENTWISE)
@@ -365,6 +392,13 @@ static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
             ZK_REQUIRE(sosp_shape_ok(l->K, l->degree),
                        "layer_create: SOSP polynomials=%d degree=%d (degree <= 15, K (degree + 1) + 1 <= 1024)", l->K, l->degree);
             ZK_REQUIRE(l->bound > 0.f, "layer_create: bisection bound=%g", (double)l->bound);
+            ZK_REQUIRE(l->iters >= 1 && l->iters <= 64, "layer_create: bisection iterations=%d (must be in [1, 64])", l->iters);
+        }
+        if (l->uni == ZK_UNI_BERNSTEIN) {  // BPF is a MAF (flows/polynomial.py:79-117): autoregressive layers only
+            if (l->kind != ZK_LAYER_AUTOREGRESSIVE)
+                return fail(ZK_EUNSUPPORTED, "layer_create: the Bernstein bijector is supported in autoregressive layers only");
+            ZK_REQUIRE(bernstein_shape_ok(l->degree), "layer_create: Bernstein degree=%d (must be in [0, 59])", l->degree);
+            ZK_REQUIRE(l->bound > 0.f, "layer_create: Bernstein bound=%g", (double)l->bound);
             ZK_REQUIRE(l->iters >= 1 && l->iters <= 64, "layer_create: bisection iterations=%d (must be in [1, 64])", l->iters);
         }
         if (l->uni == ZK_UNI_RQS) ZK_REQUIRE(l->K >= 1 && l->K <= 1024, "layer_create: bins=%d", l->K);

@@ -611,11 +611,11 @@ zk_status flow_inverse_backward_chunk(const zk_flow_desc* f, const float* x, int
 zk_status uni_backward_entry(int uni, const float* x, int64_t ldx, const float* phi, int64_t phi_ld,
                              int64_t B, int D, int K, float bound, float slope, const float* gy,
                              int64_t ldgy, const float* gl, float* gx, int64_t ldgx, float* gphi,
-                             void* ws, size_t ws_bytes, cudaStream_t st, int degree = 0) {
+                             void* ws, size_t ws_bytes, cudaStream_t st, int degree = 0, float eps = kBernsteinEps) {
     ZK_REQUIRE(x && phi && B >= 0 && D > 0, "univariate backward: bad arguments");
     const int P = uni_param_count(uni, K, degree);
     UniBwdArgs u;
-    u.univariate = uni; u.K = K; u.degree = degree; u.bound = bound; u.slope = slope; u.D = D;
+    u.univariate = uni; u.K = K; u.degree = degree; u.bound = bound; u.slope = slope; u.eps = eps; u.D = D;
     u.fast_math = g_fast_math.load() != 0;
     u.phi = phi; u.phi_ld = phi_ld;
     if (phi_ld != 0 || gphi == nullptr) {
@@ -682,6 +682,15 @@ zk_status zk_sosp_backward(const float* x, int64_t ldx, const float* phi, int64_
     ZK_REQUIRE(sosp_shape_ok(K, degree), "sosp backward: polynomials %d / degree %d out of range", K, degree);
     return uni_backward_entry(ZK_UNI_SOSP, x, ldx, phi, phi_ld, B, D, K, bound, slope, grad_y, ldgy, grad_ladj,
                               grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream, degree);
+}
+
+zk_status zk_bernstein_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
+                                int degree, float bound, float eps, const float* grad_y, int64_t ldgy,
+                                const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi, void* ws,
+                                size_t ws_bytes, zk_stream stream) {
+    ZK_REQUIRE(bernstein_shape_ok(degree), "bernstein backward: degree must be in [0, 59], got %d", degree);
+    return uni_backward_entry(ZK_UNI_BERNSTEIN, x, ldx, phi, phi_ld, B, D, 0, bound, 1e-3f, grad_y, ldgy, grad_ladj,
+                              grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream, degree, eps);
 }
 
 zk_status zk_softclip_backward(const float* x, int64_t ldx, int64_t B, int D, float bound,

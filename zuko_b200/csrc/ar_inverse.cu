@@ -10,9 +10,9 @@
 //   step p = 0 .. passes-1:
 //     every hidden unit whose inputs became final at step p is computed;
 //     the P parameter rows of every dim of class p are computed from the last hidden layer;
-//     the inverse bijector (transforms.py:534-548 / 443-444, or the SOSP bisection of
-//     transforms.py:609-617 in registers) yields x_d, which is stored and becomes an input of the
-//     later steps.
+//     the inverse bijector (transforms.py:534-548 / 443-444, or the SOSP / Bernstein bisection of
+//     transforms.py:609-617, 807-831 in registers) yields x_d, which is stored and becomes an input of
+//     the later steps.
 //
 // This visits every weight once instead of `passes` times and reproduces the reference's fixed
 // point up to summation order (SURVEY §3.2, §7.2).  The same sweep also yields what
@@ -83,6 +83,7 @@ struct InvParams {
     float sign;        // +1: accumulate the forward ladj at the solution; -1: the layer is an inverted flow member
     const float* base_loc; const float* base_scale;
     sosp::Const sosp;  // SOSP: bisection and pre-scaled quadrature of the default shape
+    bern::Const bern;  // Bernstein: order, bound, eps and bisection of the default degree
 };
 
 // two fp32 FMAs on a pair (fmaf rounding)
@@ -126,7 +127,8 @@ __device__ __forceinline__ void tile_dot(const float* __restrict__ w, const floa
 //           then per dim ONE block of its PT tiles: K x (PT * 8) weights k-major + PT * 8 biases
 template <int UNI, int KT, bool FAST, int R, bool GACT>
 __global__ void __launch_bounds__(256) ar_inverse_kernel(const InvParams p) {
-    constexpr int P = (UNI == ZK_UNI_RQS) ? 3 * KT - 1 : (UNI == ZK_UNI_SOSP ? sosp::kDefP : 2);
+    constexpr int P = (UNI == ZK_UNI_RQS) ? 3 * KT - 1
+                    : (UNI == ZK_UNI_SOSP ? sosp::kDefP : (UNI == ZK_UNI_BERNSTEIN ? bern::kDefP : 2));
     constexpr int PT = (P + TILE - 1) / TILE;  // tiles per dim
     extern __shared__ __align__(16) float state[];  // [state_floats][S], S = R * T samples
     const int T = blockDim.x;
@@ -288,6 +290,15 @@ __global__ void __launch_bounds__(256) ar_inverse_kernel(const InvParams p) {
                     } else if constexpr (UNI == ZK_UNI_SOSP) {
                         xv = sosp::inverse<KT>(phi[j], p.sosp, yv[j]);
                         lj = zlog<FAST>(sosp::g<KT>(phi[j], p.sosp, xv));  // ladj of the forward map at the solution
+                    } else if constexpr (UNI == ZK_UNI_BERNSTEIN) {
+                        constexpr int MT = bern::kDefM;
+                        float w[bern::kDefP], mx, rs;
+                        bern::softmax<bern::kDefP>(phi[j], p.bern, w, mx, rs);
+                        auto dl = [&](int q) { return bern::delta<bern::kDefP>(phi[j], w, p.bern, mx, rs, q); };
+                        xv = bern::inverse<MT>(p.bern, yv[j], dl);
+                        float fp;
+                        bern::forward<MT>(p.bern, xv, dl, &fp);
+                        lj = zlog<FAST>(fp);  // ladj of the forward map at the solution
                     } else {
                         const float ls = softclip<FAST>(phi[j][1], p.ad);
                         xv = zdiv<FAST>(yv[j] - phi[j][0], zexp<FAST>(ls));
@@ -321,7 +332,7 @@ zk_status launch_inv_t(const InvParams& p, bool fast, int R, int grid, int T, si
         kern<<<grid, T, smem, st>>>(p);
         return check_launch("ar_inverse_kernel");
     };
-    constexpr bool kTwo = UNI != ZK_UNI_SOSP;  // SOSP: one sample per thread only (inv_geometry)
+    constexpr bool kTwo = UNI != ZK_UNI_SOSP && UNI != ZK_UNI_BERNSTEIN;  // bisections: one sample per thread only (inv_geometry)
     if (p.act != 1) {  // general activation: one instantiation per sample tiling (IEEE math in the activation)
         if constexpr (kTwo)
             if (R == 2) return fast ? go(ar_inverse_kernel<UNI, KT, true, 2, true>) : go(ar_inverse_kernel<UNI, KT, false, 2, true>);
@@ -347,7 +358,7 @@ bool inv_geometry(const ArInvPack* pk, int* threads, int* per_thread, size_t* sm
     auto set = [&](int T, int R) { *threads = T; *per_thread = R; *smem = per_sample * T * R + wbytes; return true; };
     if (const char* e = getenv("ZK_INV_GEOM")) {
         int T = 0, R = 0;
-        const bool r2 = pk->uni != ZK_UNI_SOSP;  // SOSP: R = 2 would spill (two register bisections); not compiled
+        const bool r2 = pk->uni != ZK_UNI_SOSP && pk->uni != ZK_UNI_BERNSTEIN;  // R = 2 would spill (two register bisections); not compiled
         if (sscanf(e, "%dx%d", &T, &R) == 2 && (R == 1 || (R == 2 && r2)) && T >= 32 && T <= 256 && T % 32 == 0 && fits(T, R)) return set(T, R);
     }
     // two CTAs of 128 samples per SM when they fit (8 warps hide the FMA / LDS latencies of the dot
@@ -376,7 +387,8 @@ zk_status ar_inverse_pack(const zk_mlp* m, const uint8_t* const* mask_dev, const
     if (!m->plain) return ZK_OK;  // residual blocks use the sweeps
     if (uni == ZK_UNI_RQS && bins != 8 && bins != 16) return ZK_OK;
     if (uni == ZK_UNI_SOSP && (bins != sosp::kDefK || degree != sosp::kDefL)) return ZK_OK;  // compiled for P = 16 only
-    if (uni != ZK_UNI_RQS && uni != ZK_UNI_AFFINE && uni != ZK_UNI_SOSP) return ZK_OK;
+    if (uni == ZK_UNI_BERNSTEIN && degree != bern::kDefDegree) return ZK_OK;  // compiled for P = 17 only
+    if (uni != ZK_UNI_RQS && uni != ZK_UNI_AFFINE && uni != ZK_UNI_SOSP && uni != ZK_UNI_BERNSTEIN) return ZK_OK;
     if (m->dims[0] != D + C) return ZK_OK;
     const int P = uni_param_count(uni, bins, degree);
     if (m->dims[L] != D * P) return ZK_OK;
@@ -589,6 +601,11 @@ zk_status launch_ar_inverse(const ArInvPack* pk, const ArInvArgs& a, cudaStream_
     if (pk->uni == ZK_UNI_SOSP) {
         ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "ar_inverse: bisection steps must be in [1, 64], got %d", a.iters);
         return launch_inv_t<ZK_UNI_SOSP, sosp::kDefK>(p, a.fast, R, (int)grid, T, smem, st);
+    }
+    if (pk->uni == ZK_UNI_BERNSTEIN) {
+        ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "ar_inverse: bisection steps must be in [1, 64], got %d", a.iters);
+        p.bern = bern::make_const(pk->degree, a.bound, kBernsteinEps, a.iters);
+        return launch_inv_t<ZK_UNI_BERNSTEIN, bern::kDefP>(p, a.fast, R, (int)grid, T, smem, st);
     }
     return launch_inv_t<ZK_UNI_AFFINE, 0>(p, a.fast, R, (int)grid, T, smem, st);
 }

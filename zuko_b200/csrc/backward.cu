@@ -35,10 +35,16 @@ struct UniBwdParams {
 struct SospBwdParams : UniBwdParams {
     sosp::Const sosp;
 };
+// Bernstein kernels take the order, bound and eps the same way
+struct BernBwdParams : UniBwdParams {
+    bern::Const bern;
+};
 template <int UNI>
 struct BwdParamsFor { using type = UniBwdParams; };
 template <>
 struct BwdParamsFor<ZK_UNI_SOSP> { using type = SospBwdParams; };
+template <>
+struct BwdParamsFor<ZK_UNI_BERNSTEIN> { using type = BernBwdParams; };
 
 __device__ __forceinline__ float circ_shift_b(float x, float bound) {  // bijector_math.cuh:circ_shift
     const float m = 2.f * bound;
@@ -96,6 +102,15 @@ __global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const typename Bwd
                 sosp::backward_pair<KT>(ar, a.sosp, xv, gyv, glv, gxv, out);
             } else {
                 sosp::backward_pair<0>(pp, a.sosp, xv, gyv, glv, gxv, out);
+            }
+        } else if constexpr (UNI == ZK_UNI_BERNSTEIN) {
+            if constexpr (KT > 0) {  // register copy of the parameters; out may alias pp
+                float ur[bern::kDefP];
+#pragma unroll
+                for (int q = 0; q < bern::kDefP; ++q) ur[q] = pp[q];
+                bern::backward_pair<bern::kDefP>(ur, a.bern, xv, gyv, glv, gxv, out);
+            } else {
+                bern::backward_pair<0>(pp, a.bern, xv, gyv, glv, gxv, out);
             }
         } else {
             bijgrad::affine_backward_pair(pp, xv, gyv, glv, a.ad, gxv, out);
@@ -326,8 +341,9 @@ zk_status launch_uni_bwd_t(const typename BwdParamsFor<UNI>::type& p, bool fast,
         kern<<<grid, kBwdThreads, smem, st>>>(p);
         return check_launch("uni_bwd_kernel");
     };
-    // affine: one expf per pair, not worth a variant; SOSP: no transcendental in its reverse mode
-    if (fast && UNI != ZK_UNI_AFFINE && UNI != ZK_UNI_SOSP) return go(uni_bwd_kernel<UNI, KT, true>);
+    // affine: one expf per pair, not worth a variant; SOSP: no transcendental in its reverse mode;
+    // Bernstein: no approximated transcendental in its reverse mode
+    if (fast && UNI != ZK_UNI_AFFINE && UNI != ZK_UNI_SOSP && UNI != ZK_UNI_BERNSTEIN) return go(uni_bwd_kernel<UNI, KT, true>);
     return go(uni_bwd_kernel<UNI, KT, false>);
 }
 
@@ -338,7 +354,7 @@ zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate backward: null input");
     ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS ||
-                   a.univariate == ZK_UNI_SOSP,
+                   a.univariate == ZK_UNI_SOSP || a.univariate == ZK_UNI_BERNSTEIN,
                "univariate backward: unknown kind %d", a.univariate);
     if (a.univariate == ZK_UNI_RQS) {
         ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "rqs backward: bins must be in [1, 1024], got %d", a.K);
@@ -347,6 +363,10 @@ zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
     } else if (a.univariate == ZK_UNI_SOSP) {
         ZK_REQUIRE(sosp_shape_ok(a.K, a.degree), "sosp backward: polynomials %d / degree %d out of range", a.K, a.degree);
         ZK_REQUIRE(a.bound > 0.f, "sosp backward: bound must be positive");
+    } else if (a.univariate == ZK_UNI_BERNSTEIN) {
+        ZK_REQUIRE(bernstein_shape_ok(a.degree), "bernstein backward: degree must be in [0, 59], got %d", a.degree);
+        ZK_REQUIRE(a.bound > 0.f, "bernstein backward: bound must be positive");
+        ZK_REQUIRE(a.eps > 0.f && a.eps < 0.5f, "bernstein backward: eps must be in (0, 1/2), got %g", (double)a.eps);
     }
     const int P = uni_param_count(a.univariate, a.K, a.degree);
     ZK_REQUIRE(a.phi_ld == 0 || a.phi_ld >= (int64_t)a.D * P, "univariate backward: phi_ld too small");
@@ -388,6 +408,13 @@ zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
         if (a.K == sosp::kDefK && a.degree == sosp::kDefL)
             return launch_uni_bwd_t<ZK_UNI_SOSP, sosp::kDefK>(sp, a.fast_math, (int)grid, smem, stream);
         return launch_uni_bwd_t<ZK_UNI_SOSP, 0>(sp, a.fast_math, (int)grid, smem, stream);
+    }
+    if (a.univariate == ZK_UNI_BERNSTEIN) {
+        BernBwdParams bp;
+        static_cast<UniBwdParams&>(bp) = p;
+        bp.bern = bern::make_const(a.degree, a.bound, a.eps, 0);
+        if (P == bern::kDefP) return launch_uni_bwd_t<ZK_UNI_BERNSTEIN, bern::kDefP>(bp, a.fast_math, (int)grid, smem, stream);
+        return launch_uni_bwd_t<ZK_UNI_BERNSTEIN, 0>(bp, a.fast_math, (int)grid, smem, stream);
     }
     switch (a.K) {
         case 8: return launch_uni_bwd_t<ZK_UNI_RQS, 8>(p, a.fast_math, (int)grid, smem, stream);

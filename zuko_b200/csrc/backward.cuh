@@ -3,7 +3,7 @@
 // What torch.autograd does for the reference when a training loop calls
 // `(-flow(c).log_prob(x).mean()).backward()` (README.md:43-49, tests/test_flows.py:22-29),
 // re-derived per kernel:
-//   * univariate bijectors (zuko/transforms.py:469-567, 426-446, 299-316, 834-875, 878-963): uni_bwd_kernel
+//   * univariate bijectors (zuko/transforms.py:469-567, 426-446, 299-316, 834-875, 878-963, 640-831): uni_bwd_kernel
 //   * (masked) MLP conditioner (zuko/nn.py:217-218): dgrad = linear_fp32_kernel on the
 //     transposed pre-masked weights, wgrad = wgrad_fp32_kernel (split over the batch,
 //     fixed-order reduction, mask applied to the result), bias = column sums
@@ -30,7 +30,8 @@ struct UniBwdArgs {
     const int* dim_map = nullptr;
     int64_t B = 0;
     int D = 0, K = 0;
-    int degree = 0;         // SOSP: polynomial degree L (K = polynomials)
+    int degree = 0;         // SOSP: polynomial degree L (K = polynomials); Bernstein: BPF degree
+    float eps = kBernsteinEps;  // Bernstein: branch threshold on t
     float bound = 5.f, slope = 1e-3f;
     bool circular = false;  // RQS: CircularShiftTransform(bound) in front (d shift / dx = 1)
     bool fast_math = false; // MUFU reciprocal / ex2 in the RQS and Gaussianization pair math (zk_set_fast_math)

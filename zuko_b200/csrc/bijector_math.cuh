@@ -3,6 +3,7 @@
 #pragma once
 
 #include "common.cuh"
+#include "bernstein_math.cuh"
 #include "sosp_math.cuh"
 
 namespace zk {

@@ -9,7 +9,9 @@
 // ladj instead of the reference's autograd call per forward (transforms.py:623-637), and its
 // bisection inverse (transforms.py:609-617, utils.py:159-183) run in registers, and the
 // sum-of-squares polynomial bijector of SOSPF (flows/polynomial.py:23-28, sosp_math.cuh): its
-// Gauss-Legendre forward, log g(x), and the same bisection on y - constant.
+// Gauss-Legendre forward, log g(x), and the same bisection on y - constant, and the bounded Bernstein
+// bijector of BPF (transforms.py:640-831, bernstein_math.cuh): softmax, the Bernstein sums, log f'(x),
+// and the bisection of the full map between its two linear branches.
 //
 // Data movement: a CTA owns a tile of R consecutive sample rows.  Their phi block is
 // one contiguous range of R*D*P floats in HBM; it is staged into shared memory with a
@@ -52,6 +54,7 @@ struct UniParams {
     int use_bulk;  // host-side verdict: alignment rules for cp.async.bulk hold for full tiles
     int iters;     // Gaussianization inverse: bisection steps
     sosp::Const sosp;  // SOSP: shape, bisection and pre-scaled quadrature
+    bern::Const bern;  // Bernstein: order, bound, eps and bisection
 };
 
 // SOSP pair: the default shape works on a register copy of its 16 parameters (four 16-byte loads:
@@ -78,6 +81,31 @@ __device__ __forceinline__ float sosp_pair(const float* pp, const sosp::Const& c
         return run(ar);
     } else {
         return run(pp);
+    }
+}
+
+// Bernstein pair: the default degree takes its 17 parameters to registers and keeps the scaled softmax
+// there; other degrees form each softmax entry from shared memory when the sums need it
+template <int KT, bool INVERSE, bool FAST>
+__device__ __forceinline__ float bern_pair(const float* pp, const bern::Const& c, float xv, float& lj) {
+    constexpr int PT = KT > 0 ? bern::kDefP : 0;
+    constexpr int MT = KT > 0 ? bern::kDefM : 0;
+    float u[PT > 0 ? PT : 1], w[PT > 0 ? PT : 1];
+    if constexpr (PT > 0) {
+#pragma unroll
+        for (int q = 0; q < PT; ++q) u[q] = pp[q];
+    }
+    const float* up = PT > 0 ? u : pp;
+    float mx, rs;
+    bern::softmax<PT>(up, c, w, mx, rs);
+    auto dl = [&](int j) { return bern::delta<PT>(up, w, c, mx, rs, j); };
+    if constexpr (INVERSE) {
+        return bern::inverse<MT>(c, xv, dl);
+    } else {
+        float fp;
+        const float yv = bern::forward<MT>(c, xv, dl, &fp);
+        lj = zlog<FAST>(fp);
+        return yv;
     }
 }
 
@@ -148,6 +176,8 @@ __global__ void __launch_bounds__(kUniThreads) uni_kernel(const UniParams a) {
                 }
             } else if constexpr (UNI == ZK_UNI_SOSP) {
                 yv = sosp_pair<KT, INVERSE, FAST>(pp, a.sosp, xv, lj);
+            } else if constexpr (UNI == ZK_UNI_BERNSTEIN) {
+                yv = bern_pair<KT, INVERSE, FAST>(pp, a.bern, xv, lj);
             } else {  // affine, transforms.py:435-446: phi = (shift, unconstrained log-scale)
                 const float shift = pp[0];
                 const float ls = softclip<FAST>(pp[1], a.ad);
@@ -223,6 +253,10 @@ zk_status launch_uni_dir(const UniParams& p, int uni, bool fast, int grid, size_
             return launch_uni_t<ZK_UNI_SOSP, sosp::kDefK, INVERSE>(p, fast, grid, smem, st);
         return launch_uni_t<ZK_UNI_SOSP, 0, INVERSE>(p, fast, grid, smem, st);
     }
+    if (uni == ZK_UNI_BERNSTEIN) {
+        if (p.bern.P == bern::kDefP) return launch_uni_t<ZK_UNI_BERNSTEIN, bern::kDefP, INVERSE>(p, fast, grid, smem, st);
+        return launch_uni_t<ZK_UNI_BERNSTEIN, 0, INVERSE>(p, fast, grid, smem, st);
+    }
     switch (p.K) {
         case 4: return launch_uni_t<ZK_UNI_RQS, 4, INVERSE>(p, fast, grid, smem, st);
         case 8: return launch_uni_t<ZK_UNI_RQS, 8, INVERSE>(p, fast, grid, smem, st);
@@ -238,7 +272,7 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate: null input");
     ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS ||
-                   a.univariate == ZK_UNI_SOSP,
+                   a.univariate == ZK_UNI_SOSP || a.univariate == ZK_UNI_BERNSTEIN,
                "univariate: unknown kind %d", a.univariate);
     if (a.univariate == ZK_UNI_RQS) {
         ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "rqs: bins must be in [1, 1024], got %d", a.K);
@@ -251,6 +285,11 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
                    a.K, a.degree);
         ZK_REQUIRE(a.bound > 0.f, "sosp: bound must be positive");
         if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "sosp: bisection steps must be in [1, 64], got %d", a.iters);
+    } else if (a.univariate == ZK_UNI_BERNSTEIN) {
+        ZK_REQUIRE(bernstein_shape_ok(a.degree), "bernstein: degree must be in [0, 59], got %d", a.degree);
+        ZK_REQUIRE(a.bound > 0.f, "bernstein: bound must be positive");
+        ZK_REQUIRE(a.eps > 0.f && a.eps < 0.5f, "bernstein: eps must be in (0, 1/2), got %g", (double)a.eps);
+        if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "bernstein: bisection steps must be in [1, 64], got %d", a.iters);
     }
     const int P = uni_param_count(a.univariate, a.K, a.degree);
     ZK_REQUIRE(a.phi_ld == 0 || a.phi_ld >= (int64_t)a.D * P, "univariate: phi_ld too small");
@@ -266,6 +305,7 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     p.circ = (a.circular && a.univariate == ZK_UNI_RQS) ? 1 : 0;
     p.iters = a.iters;
     if (a.univariate == ZK_UNI_SOSP) p.sosp = sosp::make_const(a.K, a.degree, a.bound, a.slope, a.iters);
+    if (a.univariate == ZK_UNI_BERNSTEIN) p.bern = bern::make_const(a.degree, a.bound, a.eps, a.iters);
     const float absL = fabsf(logf(a.slope));
     p.aw = 2.f / absL;
     p.ad = 1.f / absL;

@@ -25,9 +25,10 @@ struct UniArgs {
     int64_t B = 0;
     int D = 0;      // number of transformed dims (pairs per sample)
     int K = 0;      // bins (RQS) / mixture components (Gaussianization) / polynomials (SOSP)
-    int degree = 0; // SOSP: polynomial degree L
+    int degree = 0; // SOSP: polynomial degree L; Bernstein: BPF degree (P = degree + 1)
     float bound = 5.f;
-    int iters = 0;  // Gaussianization / SOSP inverse: bisection steps on [-bound, bound]
+    int iters = 0;  // Gaussianization / SOSP / Bernstein inverse: bisection steps on [-bound, bound]
+    float eps = kBernsteinEps;  // Bernstein: branch threshold on t = (x + bound) / 2 bound
     float slope = 1e-3f;
     bool circular = false;  // RQS only: CircularShiftTransform(bound) in front (forward) / behind (inverse)
     bool fast_math = true;  // MUFU rcp/ex2/lg2 fast path (default) vs IEEE div + expf/logf

@@ -51,12 +51,13 @@ inline zk_status check_launch(const char* what) {
 int sm_count();  // cached, current device
 
 // parameters per (sample, dim) pair of a univariate bijector (ZK_UNI_*; K = bins / components /
-// polynomials, degree: ZK_UNI_SOSP only)
+// polynomials, degree: ZK_UNI_SOSP and ZK_UNI_BERNSTEIN only)
 inline int uni_param_count(int uni, int K, int degree) {
     switch (uni) {
         case ZK_UNI_RQS: return 3 * K - 1;
         case ZK_UNI_GAUSS: return 2 * K;
         case ZK_UNI_SOSP: return K * (degree + 1) + 1;
+        case ZK_UNI_BERNSTEIN: return degree + 1;
         default: return 2;
     }
 }
@@ -64,6 +65,11 @@ inline int uni_param_count(int uni, int K, int degree) {
 inline bool sosp_shape_ok(int K, int degree) {
     return K >= 1 && K <= 1023 && degree >= 0 && degree <= 15 && K * (degree + 1) + 1 <= 1024;
 }
+
+// shape limits of the bounded Bernstein bijector: order M = degree + 5 <= 64
+inline bool bernstein_shape_ok(int degree) { return degree >= 0 && degree <= 59; }
+// eps of BoundedBernsteinTransform in flow layers (zk_layer_desc carries no eps)
+constexpr float kBernsteinEps = 1e-6f;
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }

@@ -4,7 +4,7 @@ from .autoregressive import MAF, MaskedAutoregressiveTransform
 from .coupling import NICE, GeneralCouplingTransform, RealNVP
 from .elementwise import ElementWiseTransform
 from .gaussianization import GF
-from .polynomial import SOSPF
+from .polynomial import BPF, SOSPF
 from .spline import NCSF, NSF
 from ..lazy import Flow, UnconditionalDistribution, UnconditionalTransform
 
@@ -14,6 +14,7 @@ __all__ = [
     "NCSF",
     "NICE",
     "NSF",
+    "BPF",
     "SOSPF",
     "ElementWiseTransform",
     "Flow",

@@ -15,6 +15,7 @@ from .. import _engine as E
 import math
 
 from ..transforms import (
+    BoundedBernsteinTransform,
     CircularRQSTransform,
     GaussianizationTransform,
     MonotonicAffineTransform,
@@ -81,10 +82,29 @@ def resolve_univariate(univariate: Callable, shapes: Sequence[Size]) -> dict:
                                       "(the engine takes degree <= 15 and K (degree + 1) + 1 <= 1024)")  # fmt: skip
         return dict(kind=E.ZK_UNI_SOSP, bins=K, degree=n - 1, bound=10.0, slope=float(kwargs.get("slope", 1e-3)),
                     total=K * n + 1, iterations=bisection_steps(10.0, 1e-6))  # fmt: skip
+    if f is BoundedBernsteinTransform:  # flows/polynomial.py:79-117: shapes [(degree + 1,)]
+        if len(shapes) != 1 or len(shapes[0]) != 1 or shapes[0][0] < 1:
+            raise ValueError(f"BoundedBernsteinTransform expects shapes [(degree + 1,)], got {shapes}")
+        extra = set(kwargs) - {"bound", "eps"}
+        if extra:
+            raise NotImplementedError(f"zuko_b200: unsupported BoundedBernsteinTransform arguments {sorted(extra)}")
+        degree = shapes[0][0] - 1
+        bound, eps = float(kwargs.get("bound", 5.0)), float(kwargs.get("eps", 1e-6))
+        if eps != 1e-6:
+            raise NotImplementedError(f"zuko_b200: BoundedBernsteinTransform in a flow layer takes eps = 1e-6 only, got {eps}")
+        if degree > 59:
+            raise NotImplementedError(f"zuko_b200: BoundedBernsteinTransform of degree {degree} (the engine takes degree <= 59)")
+        if not bound > 0:
+            raise ValueError(f"BoundedBernsteinTransform expects a positive bound, got {bound}")
+        return dict(kind=E.ZK_UNI_BERNSTEIN, bins=0, degree=degree, bound=bound, slope=1e-3, total=degree + 1,
+                    iterations=bisection_steps(bound, eps))  # fmt: skip
+    if getattr(f, "__name__", None) == "BernsteinTransform":
+        raise NotImplementedError("zuko_b200: the unbounded BernsteinTransform is not implemented by the engine "
+                                  "(BPF uses BoundedBernsteinTransform)")  # fmt: skip
     raise NotImplementedError(
         f"zuko_b200: univariate transformation {getattr(f, '__name__', f)!r} is not implemented by the engine "
         "(supported: MonotonicAffineTransform, MonotonicRQSTransform, CircularRQSTransform, GaussianizationTransform, "
-        "ShiftedSOSPTransform)"
+        "ShiftedSOSPTransform, BoundedBernsteinTransform)"
     )
 
 
@@ -100,6 +120,8 @@ def refuse_autoregressive_only(uni: dict, layer: str) -> None:
     (flows/polynomial.py:31-76)."""
     if uni["kind"] == E.ZK_UNI_SOSP:
         raise NotImplementedError(f"zuko_b200: ShiftedSOSPTransform is supported in autoregressive layers only, not in {layer}")
+    if uni["kind"] == E.ZK_UNI_BERNSTEIN:
+        raise NotImplementedError(f"zuko_b200: BoundedBernsteinTransform is supported in autoregressive layers only, not in {layer}")
 
 
 class OwnedLayer:
@@ -240,6 +262,8 @@ class PackedLayerMixin:
                            iterations=u.get("iterations", 0), degree=u.get("degree", 0))  # fmt: skip
 
     def _describe_base(self) -> str:
+        if self._uni["kind"] == E.ZK_UNI_BERNSTEIN:
+            return "BoundedBernsteinTransform(degree=%d, bound=%g)" % (self._uni["degree"], self._uni["bound"])
         if self._uni["kind"] == E.ZK_UNI_SOSP:
             return "ShiftedSOSPTransform(polynomials=%d, degree=%d)" % (self._uni["bins"], self._uni["degree"])
         if self._uni["kind"] == E.ZK_UNI_GAUSS:

@@ -1,13 +1,14 @@
-"""Polynomial flows (zuko/flows/polynomial.py): the sum-of-squares polynomial flow."""
+"""Polynomial flows (zuko/flows/polynomial.py): the sum-of-squares polynomial flow and the Bernstein
+polynomial flow."""
 
 from __future__ import annotations
 
-__all__ = ["SOSPF", "ShiftedSOSPTransform"]
+__all__ = ["BPF", "SOSPF", "ShiftedSOSPTransform"]
 
 from functools import partial
 
 from ..lazy import UnconditionalTransform
-from ..transforms import ShiftedSOSPTransform, SoftclipTransform
+from ..transforms import BoundedBernsteinTransform, ShiftedSOSPTransform, SoftclipTransform
 from .autoregressive import MAF
 
 
@@ -41,3 +42,28 @@ class SOSPF(MAF):
 
         for i in reversed(range(1, len(transforms))):
             transforms.insert(i, UnconditionalTransform(SoftclipTransform, bound=11.0))
+
+
+class BPF(MAF):
+    """Bernstein polynomial flow: a :class:`MAF` whose univariate bijector is ``BoundedBernsteinTransform``
+    (bound 5) with ``degree + 1`` unconstrained parameters per feature.  Same arguments, module tree,
+    state-dict keys and seeded initialisation as the reference.
+
+    The polynomial acts on ``[-5, 5]``; beyond it the map is linear with slope 1 (``x -+ 1e-5``), so
+    standardise the features first, as the reference recommends.  Degree 16 inverts with the
+    dimension-sequential kernel, other degrees with the ``passes`` sweeps."""
+
+    def __init__(
+        self,
+        features: int,
+        context: int = 0,
+        degree: int = 16,
+        **kwargs,
+    ) -> None:
+        super().__init__(
+            features=features,
+            context=context,
+            univariate=BoundedBernsteinTransform,
+            shapes=[(degree + 1,)],
+            **kwargs,
+        )

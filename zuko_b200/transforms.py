@@ -8,7 +8,8 @@ C ABI of the H100 engine; no torch arithmetic runs here.
 * univariate bijectors built from explicit parameters:
   ``MonotonicRQSTransform`` (transforms.py:449-567), ``MonotonicAffineTransform``
   (:412-446), ``GaussianizationTransform`` (:834-875), ``SOSPolynomialTransform`` (:931-963,
-  with ``ShiftedSOSPTransform`` of zuko/flows/polynomial.py:23-28), ``SoftclipTransform`` (:286-316);
+  with ``ShiftedSOSPTransform`` of zuko/flows/polynomial.py:23-28), ``BoundedBernsteinTransform``
+  (:640-831), ``SoftclipTransform`` (:286-316);
 * linear maps: ``PermutationTransform`` (:1182-1214), ``RotationTransform`` (:1217-1244);
 * packed conditional layers produced by the lazy modules in ``zuko_b200.flows``:
   ``AutoregressiveTransform`` (:966-1007), ``CouplingTransform`` (:1010-1073),
@@ -20,6 +21,7 @@ C ABI of the H100 engine; no torch arithmetic runs here.
 from __future__ import annotations
 
 __all__ = [
+    "BoundedBernsteinTransform",
     "AutoregressiveTransform",
     "CircularRQSTransform",
     "CircularShiftTransform",
@@ -159,6 +161,9 @@ def _uni_forward(kind: int, K: int, bound: float, slope: float, x2: Tensor, phi:
         elif kind == E.ZK_UNI_SOSP:
             (K, deg) = K
             E.check(L.zk_sosp_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, K, deg, bound, slope, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
+        elif kind == E.ZK_UNI_BERNSTEIN:
+            (deg, eps) = K
+            E.check(L.zk_bernstein_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, deg, bound, eps, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
         elif kind == E.ZK_UNI_AFFINE:
             E.check(L.zk_affine_forward(x2.data_ptr(), 1, phi.detach().data_ptr(), ld, N, 1, slope, y.data_ptr(), 1, ladj.data_ptr(), 0, st))
         else:
@@ -169,8 +174,9 @@ def _uni_forward(kind: int, K: int, bound: float, slope: float, x2: Tensor, phi:
 class _UniFunction(torch.autograd.Function):
     """Autograd seam of the explicit-parameter bijectors: backward = ``zk_rqs_backward`` /
     ``zk_affine_backward`` / ``zk_gaussianization_backward`` / ``zk_sosp_backward`` / ``zk_softclip_backward``
-    (reverse mode of transforms.py:469-567, 426-446, 834-875, 878-963, 299-316).  ``K`` is the pair
-    ``(polynomials, degree)`` for the sum-of-squares polynomial bijector."""
+    / ``zk_bernstein_backward`` (reverse mode of transforms.py:469-567, 426-446, 834-875, 878-963, 299-316,
+    640-831).  ``K`` is the pair ``(polynomials, degree)`` for the sum-of-squares polynomial bijector and
+    ``(degree, eps)`` for the bounded Bernstein bijector."""
 
     @staticmethod
     def forward(ctx, kind, K, bound, slope, ld, x2, phi):  # noqa: ANN001
@@ -210,6 +216,8 @@ class _UniFunction(torch.autograd.Function):
                 E.check(L.zk_gaussianization_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, K, *args))
             elif kind == E.ZK_UNI_SOSP:
                 E.check(L.zk_sosp_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, *K, bound, slope, *args))
+            elif kind == E.ZK_UNI_BERNSTEIN:
+                E.check(L.zk_bernstein_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, K[0], bound, K[1], *args))
             else:
                 E.check(L.zk_affine_backward(x2.data_ptr(), 1, phi.data_ptr(), ld, N, 1, slope, *args))
         return None, None, None, None, None, gx, gphi
@@ -390,6 +398,42 @@ def ShiftedSOSPTransform(a: Tensor, constant: Tensor, slope: float = 1e-3) -> Tr
     EngineTransform.__init__(t)
     t._setup(a, constant, slope, 10.0, 1e-6)
     return t
+
+
+class BoundedBernsteinTransform(EngineTransform):
+    """Bounded Bernstein polynomial bijector of BPF with unconstrained parameters ``theta`` of shape
+    ``(*, degree + 1)`` (zuko/transforms.py:780-831): the coefficients rise from ``-bound`` to ``bound``
+    through a softmax, the polynomial of order ``degree + 5`` maps ``[-bound, bound]`` onto itself, and two
+    linear branches of slope 1 continue it beyond (``x -+ 2 bound eps``).  ``zk_bernstein_forward`` evaluates
+    it and ``ladj = log f'(x)``; the inverse returns the linear branches for ``|y| >= bound`` and otherwise
+    runs the reference's ``ceil(log2(2 bound / eps))`` bisection steps on ``[-bound, bound]``
+    (``zk_bernstein_inverse``).  Gradients: ``zk_bernstein_backward``."""
+
+    domain = constraints.real
+    codomain = constraints.real
+
+    def __init__(self, theta: Tensor, bound: float = 5.0, eps: float = 1e-6) -> None:
+        super().__init__()
+        self.phi = theta
+        self.degree = theta.shape[-1] - 1
+        self.bound, self.eps = float(bound), float(eps)
+
+    def __repr__(self) -> str:
+        return f"{type(self).__name__}(degree={self.degree}, bound={self.bound})"
+
+    def call_and_ladj(self, x: Tensor) -> tuple[Tensor, Tensor]:
+        x2, phi, ld, shape = _elementwise(self.phi, x, self.degree + 1)
+        y, ladj = _uni_call(E.ZK_UNI_BERNSTEIN, (self.degree, self.eps), self.bound, 1e-3, x2, phi, ld)
+        return y.reshape(shape), ladj.reshape(shape)
+
+    def _inverse(self, y: Tensor) -> Tensor:
+        _no_grad_inverse(y, self.phi)
+        y2, phi, ld, shape = _elementwise(self.phi.detach(), y.detach(), self.degree + 1)
+        x = torch.empty_like(y2)
+        with torch.cuda.device(y2.device):
+            E.check(E.lib().zk_bernstein_inverse(y2.data_ptr(), 1, phi.data_ptr(), ld, y2.shape[0], 1, self.degree,
+                                                 self.bound, self.eps, x.data_ptr(), 1, E.stream_ptr(y2.device)))  # fmt: skip
+        return x.reshape(shape)
 
 
 class SoftclipTransform(EngineTransform):
