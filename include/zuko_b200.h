@@ -99,11 +99,23 @@ zk_status zk_device_info(int* sm_count, int* cc_major, int* cc_minor);
  * `ladj` is per SAMPLE: sum over D of log|dy/dx| — i.e. what
  * DependentTransform.call_and_ladj returns (transforms.py:210-214); with
  * accumulate != 0 it is added to the buffer (transforms.py:147).
- * `phi_ld` is the row stride of phi in elements (D*P for per-sample parameters
- * as produced by MaskedAutoregressiveTransform.meta, flows/autoregressive.py:
- * 207-215; 0 for one shared (D, P) table, flows/gaussianization.py:74-77).
+ * `phi_ld` is the row stride of phi in elements: D*P for dense per-sample
+ * parameters as produced by MaskedAutoregressiveTransform.meta (flows/
+ * autoregressive.py:207-215), any larger value for padded rows (the pads are
+ * never read), or 0 for one shared (D, P) table (flows/gaussianization.py:74-77).
  * y may alias x; y or ladj may be NULL when not needed.
  * ------------------------------------------------------------------------- */
+
+/* Tile plan of the stand-alone bijector kernel for these arguments, as the next launch would choose it (univariate is
+ * ZK_UNI_AFFINE, _RQS, _GAUSS, _SOSP or _BERNSTEIN; K = bins / components / polynomials; degree of SOSP / Bernstein;
+ * phi only for its alignment).  Returns ZK_OK and fills the non-NULL outputs, or the status the launch would return for
+ * these arguments.  rows_per_tile: sample rows per CTA; smem: dynamic shared memory bytes; bulk_staging: 1 when full
+ * tiles stage phi with one bulk copy; shuffle_sum: 1 when the ladj sum over D is the warp-shuffle reduction (D <= 32, a
+ * power of two), 0 for the fixed-order one; bins_instantiated: the compile-time shape the launch picks (RQS 4, 8 or 16,
+ * Gaussianization 8 or 16, SOSP 3 for (K, degree) = (3, 4), Bernstein 17 for degree 16; 0 for the runtime-shape
+ * kernel).  B = 0 reports 0 everywhere.  Read-only, no device work. */
+zk_status zk_univariate_plan(int univariate, int64_t B, int D, int K, int degree, int64_t phi_ld, const float* phi,
+                             int* rows_per_tile, size_t* smem, int* bulk_staging, int* shuffle_sum, int* bins_instantiated);
 
 /* MonotonicRQSTransform(*phi).call_and_ladj(x)   — transforms.py:469-490,554-567 */
 zk_status zk_rqs_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,

@@ -121,6 +121,12 @@ def linear(x, c, W, mask, b, relu: bool, dtype=np.float64) -> np.ndarray:
     return y
 
 
+def _check_bins(bins: int) -> None:
+    # the C restatement keeps each spline's knots in fixed stack arrays
+    if not 1 <= bins <= lib().zo_max_bins():
+        raise ValueError(f"oracle: bins={bins} outside [1, {lib().zo_max_bins()}]")
+
+
 def _phi_args(phi, B, D, P, dtype):
     phi = _c(phi, dtype)
     if phi.size == D * P:  # shared per-dimension table (gaussianization.py:74-77)
@@ -132,6 +138,7 @@ def _phi_args(phi, B, D, P, dtype):
 def rqs_forward(x, phi, bins: int, bound=5.0, slope=1e-3, dtype=np.float64):
     """MonotonicRQSTransform(*unpack(phi)).call_and_ladj(x) — transforms.py:469-567.
     Returns (y, ladj) both (B, D); ladj is per element (not summed)."""
+    _check_bins(bins)
     x = _c(x, dtype)
     B, D = x.shape
     P = 3 * bins - 1
@@ -148,6 +155,7 @@ def rqs_forward(x, phi, bins: int, bound=5.0, slope=1e-3, dtype=np.float64):
 
 def rqs_inverse(y, phi, bins: int, bound=5.0, slope=1e-3, dtype=np.float64):
     """MonotonicRQSTransform(*unpack(phi))._inverse(y) — transforms.py:534-548."""
+    _check_bins(bins)
     y = _c(y, dtype)
     B, D = y.shape
     P = 3 * bins - 1
@@ -163,6 +171,7 @@ def rqs_inverse(y, phi, bins: int, bound=5.0, slope=1e-3, dtype=np.float64):
 
 def rqs_knots(phi, bins: int, bound=5.0, slope=1e-3, dtype=np.float64):
     """(horizontal, vertical, derivatives) of transforms.py:488-490 for phi (..., 3K-1)."""
+    _check_bins(bins)
     phi = _c(phi, dtype)
     lead = phi.shape[:-1]
     n = int(np.prod(lead)) if lead else 1

@@ -9,7 +9,7 @@
 #include <stddef.h>
 #include <stdlib.h>
 
-#define ZO_MAX_BINS 256
+#define ZO_MAX_BINS 1024 /* the engine's RQS limit (bins in [1, 1024]); the knot arrays live on the stack */
 
 #define REAL float
 #define SUFFIX _f32

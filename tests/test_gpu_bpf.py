@@ -239,8 +239,8 @@ def test_lazy_inverse_member(device):
 
 @pytest.mark.parametrize("degree", [16, 7])
 def test_entry_points_strided_shared_and_empty(device, degree):
-    """zk_bernstein_forward / inverse / backward on strided rows (pads untouched; padded parameter rows in the
-    backward, which reads phi_ld), a shared row (phi_ld = 0) and B = 0, against the fp64 restatement."""
+    """zk_bernstein_forward / inverse / backward on strided rows (pads untouched; NaN-padded parameter rows, phi_ld =
+    D P + 5), a shared row (phi_ld = 0) and B = 0, against the fp64 restatement."""
     L, st = E.lib(), E.stream_ptr(device)
     B, D, P, bound, eps = 37, 3, degree + 1, 4.0, 1e-5
     g = torch.Generator().manual_seed(degree)
@@ -253,15 +253,14 @@ def test_entry_points_strided_shared_and_empty(device, degree):
     ud[:, : D * P] = u.to(device)
     yd = torch.full((B, ldx), float("nan"), device=device)
     ladj = torch.zeros(B, device=device)
-    uc = u.to(device).contiguous()  # the forward and inverse take dense parameter rows (phi_ld = D P)
-    E.check(L.zk_bernstein_forward(xd.data_ptr(), ldx, uc.data_ptr(), D * P, B, D, degree, bound, eps, yd.data_ptr(), ldx,
+    E.check(L.zk_bernstein_forward(xd.data_ptr(), ldx, ud.data_ptr(), ldp, B, D, degree, bound, eps, yd.data_ptr(), ldx,
                                    ladj.data_ptr(), 0, st))  # fmt: skip
     y64, l64 = R.forward(x.double().numpy(), u.double().numpy().reshape(B, D, P), bound, eps)
     np.testing.assert_allclose(cpu(yd[:, :D]), y64, rtol=0, atol=2e-5 * bound)
     np.testing.assert_allclose(cpu(ladj), l64.sum(-1), rtol=0, atol=1e-4)
     assert torch.isnan(yd[:, D:]).all()
     xi = torch.full((B, ldx), float("nan"), device=device)
-    E.check(L.zk_bernstein_inverse(yd.data_ptr(), ldx, uc.data_ptr(), D * P, B, D, degree, bound, eps, xi.data_ptr(), ldx, st))
+    E.check(L.zk_bernstein_inverse(yd.data_ptr(), ldx, ud.data_ptr(), ldp, B, D, degree, bound, eps, xi.data_ptr(), ldx, st))
     np.testing.assert_allclose(cpu(xi[:, :D]), x.numpy(), rtol=0, atol=1e-4)
     assert torch.isnan(xi[:, D:]).all()
     # shared row

@@ -119,6 +119,8 @@ _SIGNATURES = {
     "zk_sosp_inverse": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_int, c_float, c_float, c_int, _P, c_int64, _P]),
     "zk_bernstein_forward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_float, c_float, _P, c_int64, _P, c_int, _P]),
     "zk_bernstein_inverse": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_float, c_float, _P, c_int64, _P]),
+    "zk_univariate_plan": (c_int, [c_int, c_int64, c_int, c_int, c_int, c_int64, _P, POINTER(c_int), POINTER(c_size_t), POINTER(c_int),
+                                   POINTER(c_int), POINTER(c_int)]),
     "zk_softclip_forward": (c_int, [_P, c_int64, c_int64, c_int, c_float, _P, c_int64, _P, c_int, _P]),
     "zk_softclip_inverse": (c_int, [_P, c_int64, c_int64, c_int, c_float, _P, c_int64, _P]),
     "zk_permute": (c_int, [_P, c_int64, _P, c_int64, c_int, _P, c_int64, _P]),

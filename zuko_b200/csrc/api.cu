@@ -70,6 +70,18 @@ zk_status zk_device_info(int* sm, int* major, int* minor) {
 // ---------------------------------------------------------------------------
 // stand-alone bijectors
 // ---------------------------------------------------------------------------
+zk_status zk_univariate_plan(int univariate, int64_t B, int D, int K, int degree, int64_t phi_ld, const float* phi,
+                             int* rows_per_tile, size_t* smem, int* bulk_staging, int* shuffle_sum, int* bins_instantiated) {
+    UniPlan p;
+    ZK_TRY(uni_plan(univariate, B, D, K, degree, phi_ld, phi, p));
+    if (rows_per_tile) *rows_per_tile = p.rows_per_tile;
+    if (smem) *smem = p.smem;
+    if (bulk_staging) *bulk_staging = p.bulk ? 1 : 0;
+    if (shuffle_sum) *shuffle_sum = p.shuffle ? 1 : 0;
+    if (bins_instantiated) *bins_instantiated = p.kt;
+    return ZK_OK;
+}
+
 zk_status zk_rqs_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
                          int D, int K, float bound, float slope, float* y, int64_t ldy, float* ladj,
                          int accumulate, zk_stream stream) {

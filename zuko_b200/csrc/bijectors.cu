@@ -13,10 +13,12 @@
 // bijector of BPF (transforms.py:640-831, bernstein_math.cuh): softmax, the Bernstein sums, log f'(x),
 // and the bisection of the full map between its two linear branches.
 //
-// Data movement: a CTA owns a tile of R consecutive sample rows.  Their phi block is
-// one contiguous range of R*D*P floats in HBM; it is staged into shared memory with a
-// single 1-D TMA bulk copy (cp.async.bulk, mbarrier complete_tx) — or with coalesced
-// loads when the 16-byte alignment rules of the bulk copy do not hold.  Thread t then
+// Data movement: a CTA owns a tile of R consecutive sample rows.  With dense rows
+// (phi_ld = D*P) their phi block is one contiguous range of R*D*P floats in HBM; it is
+// staged into shared memory with a single 1-D TMA bulk copy (cp.async.bulk, mbarrier
+// complete_tx) — or with coalesced loads when the 16-byte alignment rules of the bulk copy
+// do not hold.  Padded rows (phi_ld > D*P) are gathered row by row with coalesced loads
+// into the same dense layout.  The tile plan is uni_plan's (zk_univariate_plan).  Thread t then
 // owns pair (row = t / D, dim = t % D): its P parameters sit at smem word t*P (P = 3K-1
 // is odd for even K => conflict-free), x / y are accessed coalesced, and the per-sample
 // sum over D is a warp-shuffle reduction (D a power of two <= 32) or a fixed-order
@@ -136,8 +138,15 @@ __global__ void __launch_bounds__(kUniThreads) uni_kernel(const UniParams a) {
             mbar_arrive_expect_tx(&bar, bytes);
             bulk_g2s(s_phi, g_phi, bytes, &bar);
         }
-    } else {
+    } else if (shared_tbl || a.phi_ld == (int64_t)D * P) {
         for (int i = tid; i < n_phi; i += kUniThreads) s_phi[i] = g_phi[i];
+    } else {  // padded rows: row r of the tile starts at g_phi + r * phi_ld and lands dense at s_phi + r * D * P
+        const int row_len = D * P;
+#pragma unroll 1
+        for (int i = tid; i < n_phi; i += kUniThreads) {
+            const int r = i / row_len;
+            s_phi[i] = g_phi[r * a.phi_ld + (i - r * row_len)];
+        }
     }
     __syncthreads();
     if (bulk) mbar_wait(&bar, 0);
@@ -226,9 +235,9 @@ __global__ void __launch_bounds__(kUniThreads) uni_kernel(const UniParams a) {
 }
 
 template <int UNI, int KT, bool INVERSE>
-zk_status launch_uni_t(const UniParams& p, bool fast, int grid, size_t smem, cudaStream_t st) {
+zk_status launch_uni_t(const UniParams& p, bool fast, int grid, size_t smem, bool smem_attr, cudaStream_t st) {
     auto go = [&](auto kern) -> zk_status {
-        if (smem + 2048 > 48 * 1024)  // static smem (barrier) counts against the 48 KB default
+        if (smem_attr)
             ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, kUniThreads, smem, st>>>(p);
         return check_launch("uni_kernel");
@@ -237,62 +246,98 @@ zk_status launch_uni_t(const UniParams& p, bool fast, int grid, size_t smem, cud
     return go(uni_kernel<UNI, KT, INVERSE, false>);
 }
 
+// kt: the compile-time shape uni_plan picked (UniPlan::kt)
 template <bool INVERSE>
-zk_status launch_uni_dir(const UniParams& p, int uni, bool fast, int grid, size_t smem,
+zk_status launch_uni_dir(const UniParams& p, int uni, int kt, bool fast, int grid, size_t smem, bool smem_attr,
                          cudaStream_t st) {
-    if (uni == ZK_UNI_AFFINE) return launch_uni_t<ZK_UNI_AFFINE, 0, INVERSE>(p, fast, grid, smem, st);
+    if (uni == ZK_UNI_AFFINE) return launch_uni_t<ZK_UNI_AFFINE, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
     if (uni == ZK_UNI_GAUSS) {
-        switch (p.K) {
-            case 8: return launch_uni_t<ZK_UNI_GAUSS, 8, INVERSE>(p, fast, grid, smem, st);
-            case 16: return launch_uni_t<ZK_UNI_GAUSS, 16, INVERSE>(p, fast, grid, smem, st);
-            default: return launch_uni_t<ZK_UNI_GAUSS, 0, INVERSE>(p, fast, grid, smem, st);
+        switch (kt) {
+            case 8: return launch_uni_t<ZK_UNI_GAUSS, 8, INVERSE>(p, fast, grid, smem, smem_attr, st);
+            case 16: return launch_uni_t<ZK_UNI_GAUSS, 16, INVERSE>(p, fast, grid, smem, smem_attr, st);
+            default: return launch_uni_t<ZK_UNI_GAUSS, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
         }
     }
     if (uni == ZK_UNI_SOSP) {
-        if (p.sosp.K == sosp::kDefK && p.sosp.L == sosp::kDefL)
-            return launch_uni_t<ZK_UNI_SOSP, sosp::kDefK, INVERSE>(p, fast, grid, smem, st);
-        return launch_uni_t<ZK_UNI_SOSP, 0, INVERSE>(p, fast, grid, smem, st);
+        if (kt == sosp::kDefK) return launch_uni_t<ZK_UNI_SOSP, sosp::kDefK, INVERSE>(p, fast, grid, smem, smem_attr, st);
+        return launch_uni_t<ZK_UNI_SOSP, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
     }
     if (uni == ZK_UNI_BERNSTEIN) {
-        if (p.bern.P == bern::kDefP) return launch_uni_t<ZK_UNI_BERNSTEIN, bern::kDefP, INVERSE>(p, fast, grid, smem, st);
-        return launch_uni_t<ZK_UNI_BERNSTEIN, 0, INVERSE>(p, fast, grid, smem, st);
+        if (kt == bern::kDefP) return launch_uni_t<ZK_UNI_BERNSTEIN, bern::kDefP, INVERSE>(p, fast, grid, smem, smem_attr, st);
+        return launch_uni_t<ZK_UNI_BERNSTEIN, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
     }
-    switch (p.K) {
-        case 4: return launch_uni_t<ZK_UNI_RQS, 4, INVERSE>(p, fast, grid, smem, st);
-        case 8: return launch_uni_t<ZK_UNI_RQS, 8, INVERSE>(p, fast, grid, smem, st);
-        case 16: return launch_uni_t<ZK_UNI_RQS, 16, INVERSE>(p, fast, grid, smem, st);
-        default: return launch_uni_t<ZK_UNI_RQS, 0, INVERSE>(p, fast, grid, smem, st);
+    switch (kt) {
+        case 4: return launch_uni_t<ZK_UNI_RQS, 4, INVERSE>(p, fast, grid, smem, smem_attr, st);
+        case 8: return launch_uni_t<ZK_UNI_RQS, 8, INVERSE>(p, fast, grid, smem, smem_attr, st);
+        case 16: return launch_uni_t<ZK_UNI_RQS, 16, INVERSE>(p, fast, grid, smem, smem_attr, st);
+        default: return launch_uni_t<ZK_UNI_RQS, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
     }
 }
 
 }  // namespace
 
+zk_status uni_plan(int uni, int64_t B, int D, int K, int degree, int64_t phi_ld, const float* phi, UniPlan& out) {
+    ZK_REQUIRE(B >= 0 && D > 0, "univariate: bad shape B=%lld D=%d", (long long)B, D);
+    out = UniPlan{};
+    if (B == 0) return ZK_OK;
+    ZK_REQUIRE(uni == ZK_UNI_AFFINE || uni == ZK_UNI_RQS || uni == ZK_UNI_GAUSS || uni == ZK_UNI_SOSP || uni == ZK_UNI_BERNSTEIN,
+               "univariate: unknown kind %d", uni);
+    if (uni == ZK_UNI_RQS) {
+        ZK_REQUIRE(K >= 1 && K <= 1024, "rqs: bins must be in [1, 1024], got %d", K);
+        out.kt = (K == 4 || K == 8 || K == 16) ? K : 0;
+    } else if (uni == ZK_UNI_GAUSS) {
+        ZK_REQUIRE(K >= 1 && K <= 1024, "gaussianization: components must be in [1, 1024], got %d", K);
+        out.kt = (K == 8 || K == 16) ? K : 0;
+    } else if (uni == ZK_UNI_SOSP) {
+        ZK_REQUIRE(sosp_shape_ok(K, degree), "sosp: polynomials %d / degree %d out of range (degree <= 15, K (degree + 1) + 1 <= 1024)",
+                   K, degree);
+        out.kt = (K == sosp::kDefK && degree == sosp::kDefL) ? sosp::kDefK : 0;
+    } else if (uni == ZK_UNI_BERNSTEIN) {
+        ZK_REQUIRE(bernstein_shape_ok(degree), "bernstein: degree must be in [0, 59], got %d", degree);
+        out.kt = (degree + 1 == bern::kDefP) ? bern::kDefP : 0;
+    }
+    const int P = uni_param_count(uni, K, degree);
+    ZK_REQUIRE(phi_ld == 0 || phi_ld >= (int64_t)D * P, "univariate: phi_ld too small");
+
+    // tile = R rows: aim at >= 256 pairs and ~24 KB of phi per CTA, bounded by shared memory
+    const size_t row_bytes = (size_t)D * P * 4;
+    const size_t kMaxSmem = 200 * 1024;
+    ZK_REQUIRE(row_bytes + D * 4 <= kMaxSmem, "univariate: D*P too large for one tile (%zu B)", row_bytes);
+    int64_t R = (int64_t)(24 * 1024 / row_bytes);
+    const int64_t r_pairs = ceil_div(kUniThreads, D);
+    if (R < r_pairs) R = r_pairs;
+    while (R > 1 && R * (row_bytes + (size_t)D * 4) > 96 * 1024) --R;
+    if (R < 1) R = 1;
+    if (R > B) R = B;
+    const int64_t grid = ceil_div(B, R);
+    ZK_REQUIRE(grid <= 0x7fffffff, "univariate: batch too large for one launch");
+    out.rows_per_tile = (int)R;
+    out.grid = (int)grid;
+    const bool contiguous = (phi_ld == (int64_t)D * P);
+    out.bulk = contiguous && (((uintptr_t)phi) % 16 == 0) && ((R * row_bytes) % 16 == 0);
+    out.smem = (phi_ld == 0 ? row_bytes : R * row_bytes) + (size_t)R * D * 4;
+    out.smem_attr = out.smem + 2048 > 48 * 1024;  // static smem (barrier) counts against the 48 KB default
+    out.shuffle = D <= 32 && (D & (D - 1)) == 0;
+    return ZK_OK;
+}
+
 zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     ZK_REQUIRE(a.B >= 0 && a.D > 0, "univariate: bad shape B=%lld D=%d", (long long)a.B, a.D);
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate: null input");
-    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS ||
-                   a.univariate == ZK_UNI_SOSP || a.univariate == ZK_UNI_BERNSTEIN,
-               "univariate: unknown kind %d", a.univariate);
-    if (a.univariate == ZK_UNI_RQS) {
-        ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "rqs: bins must be in [1, 1024], got %d", a.K);
-    } else if (a.univariate == ZK_UNI_GAUSS) {
-        ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "gaussianization: components must be in [1, 1024], got %d", a.K);
+    UniPlan plan;
+    ZK_TRY(uni_plan(a.univariate, a.B, a.D, a.K, a.degree, a.phi_ld, a.phi, plan));
+    if (a.univariate == ZK_UNI_GAUSS) {
         ZK_REQUIRE(a.bound > 0.f, "gaussianization: bound must be positive");
         if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "gaussianization: bisection steps must be in [1, 64], got %d", a.iters);
     } else if (a.univariate == ZK_UNI_SOSP) {
-        ZK_REQUIRE(sosp_shape_ok(a.K, a.degree), "sosp: polynomials %d / degree %d out of range (degree <= 15, K (degree + 1) + 1 <= 1024)",
-                   a.K, a.degree);
         ZK_REQUIRE(a.bound > 0.f, "sosp: bound must be positive");
         if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "sosp: bisection steps must be in [1, 64], got %d", a.iters);
     } else if (a.univariate == ZK_UNI_BERNSTEIN) {
-        ZK_REQUIRE(bernstein_shape_ok(a.degree), "bernstein: degree must be in [0, 59], got %d", a.degree);
         ZK_REQUIRE(a.bound > 0.f, "bernstein: bound must be positive");
         ZK_REQUIRE(a.eps > 0.f && a.eps < 0.5f, "bernstein: eps must be in (0, 1/2), got %g", (double)a.eps);
         if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "bernstein: bisection steps must be in [1, 64], got %d", a.iters);
     }
-    const int P = uni_param_count(a.univariate, a.K, a.degree);
-    ZK_REQUIRE(a.phi_ld == 0 || a.phi_ld >= (int64_t)a.D * P, "univariate: phi_ld too small");
     ZK_REQUIRE(a.slope > 0.f && a.slope < 1.f, "univariate: slope must be in (0, 1)");
     if (a.inverse) ZK_REQUIRE(a.y != nullptr, "univariate inverse: null output");
     if (a.accumulate) ZK_REQUIRE(a.ladj != nullptr, "univariate: accumulate needs ladj");
@@ -301,7 +346,8 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     p.x = a.x; p.ldx = a.ldx; p.phi = a.phi; p.phi_ld = a.phi_ld;
     p.y = a.y; p.ldy = a.ldy; p.ladj = a.ladj; p.accumulate = a.accumulate;
     p.log_prob = a.log_prob; p.base_loc = a.base_loc; p.base_scale = a.base_scale;
-    p.dim_map = a.dim_map; p.B = a.B; p.D = a.D; p.K = a.K; p.P = P; p.bound = a.bound;
+    p.dim_map = a.dim_map; p.B = a.B; p.D = a.D; p.K = a.K; p.P = uni_param_count(a.univariate, a.K, a.degree);
+    p.bound = a.bound;
     p.circ = (a.circular && a.univariate == ZK_UNI_RQS) ? 1 : 0;
     p.iters = a.iters;
     if (a.univariate == ZK_UNI_SOSP) p.sosp = sosp::make_const(a.K, a.degree, a.bound, a.slope, a.iters);
@@ -309,25 +355,11 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     const float absL = fabsf(logf(a.slope));
     p.aw = 2.f / absL;
     p.ad = 1.f / absL;
-
-    // tile = R rows: aim at >= 256 pairs and ~24 KB of phi per CTA, bounded by shared memory
-    const size_t row_bytes = (size_t)a.D * P * 4;
-    const size_t kMaxSmem = 200 * 1024;
-    ZK_REQUIRE(row_bytes + a.D * 4 <= kMaxSmem, "univariate: D*P too large for one tile (%zu B)", row_bytes);
-    int64_t R = (int64_t)(24 * 1024 / row_bytes);
-    const int64_t r_pairs = ceil_div(kUniThreads, a.D);
-    if (R < r_pairs) R = r_pairs;
-    while (R > 1 && R * (row_bytes + (size_t)a.D * 4) > 96 * 1024) --R;
-    if (R < 1) R = 1;
-    if (R > a.B) R = a.B;
-    p.rows_per_tile = (int)R;
-    const bool contiguous = (a.phi_ld == (int64_t)a.D * P);
-    p.use_bulk = contiguous && (((uintptr_t)a.phi) % 16 == 0) && ((R * row_bytes) % 16 == 0);
-    const size_t smem = (a.phi_ld == 0 ? row_bytes : R * row_bytes) + (size_t)R * a.D * 4;
-    const int64_t grid = ceil_div(a.B, R);
-    ZK_REQUIRE(grid <= 0x7fffffff, "univariate: batch too large for one launch");
-    if (a.inverse) return launch_uni_dir<true>(p, a.univariate, a.fast_math, (int)grid, smem, stream);
-    return launch_uni_dir<false>(p, a.univariate, a.fast_math, (int)grid, smem, stream);
+    p.rows_per_tile = plan.rows_per_tile;
+    p.use_bulk = plan.bulk ? 1 : 0;
+    if (a.inverse)
+        return launch_uni_dir<true>(p, a.univariate, plan.kt, a.fast_math, plan.grid, plan.smem, plan.smem_attr, stream);
+    return launch_uni_dir<false>(p, a.univariate, plan.kt, a.fast_math, plan.grid, plan.smem, plan.smem_attr, stream);
 }
 
 // ---------------------------------------------------------------------------

@@ -13,7 +13,7 @@ struct UniArgs {
     const float* x = nullptr;  // input (B, *) ; forward: x, inverse: y
     int64_t ldx = 0;
     const float* phi = nullptr;
-    int64_t phi_ld = 0;  // elements per sample row of phi (0 = shared table)
+    int64_t phi_ld = 0;  // row stride of phi in elements, >= D*P (padded rows allowed); 0 = one shared table
     float* y = nullptr;  // output (B, *), may be null (forward + log_prob only)
     int64_t ldy = 0;
     float* ladj = nullptr;  // (B) summed over dims; forward only; may be null
@@ -34,6 +34,18 @@ struct UniArgs {
     bool fast_math = true;  // MUFU rcp/ex2/lg2 fast path (default) vs IEEE div + expf/logf
 };
 
+// Tile plan of uni_kernel (launch_univariate and zk_univariate_plan both take it from uni_plan).
+struct UniPlan {
+    int rows_per_tile = 0;   // R: >= ceil(256 / D) rows and ~24 KB of phi, shrunk to <= 96 KB, capped by B
+    int grid = 0;            // ceil(B / R) CTAs
+    size_t smem = 0;         // dynamic shared memory: phi (R rows, or one shared table) + R*D reduction floats
+    bool smem_attr = false;  // smem + the static barrier exceed the 48 KB default: raise the attribute
+    bool bulk = false;       // cp.async.bulk for full tiles: dense rows, 16-byte aligned phi and tile
+    bool shuffle = false;    // D <= 32 and a power of two: warp-shuffle ladj sum, else the fixed-order sum
+    int kt = 0;              // compile-time shape of the instantiation: RQS 4 / 8 / 16, GAUSS 8 / 16, SOSP 3, Bernstein 17
+};
+// Validates the shape arguments as launch_univariate does and fills `out`; B = 0 leaves it zero.  Host only.
+zk_status uni_plan(int uni, int64_t B, int D, int K, int degree, int64_t phi_ld, const float* phi, UniPlan& out);
 zk_status launch_univariate(const UniArgs& a, cudaStream_t stream);
 
 zk_status launch_softclip(const float* x, int64_t ldx, int64_t B, int D, float bound, bool inverse,
