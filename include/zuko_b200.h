@@ -219,7 +219,9 @@ zk_status zk_mlp_create(const zk_mlp_desc* desc, zk_mlp** out);
 zk_status zk_mlp_destroy(zk_mlp* mlp);
 size_t zk_mlp_workspace_bytes(const zk_mlp* mlp, int64_t B);
 /* out = mlp(cat(x, c)): x (B, dx), c (B, dc) or one row (ldc = 0) or NULL (dc = 0);
- * dx + dc must equal dims[0]; out is (B, dims[n_linear]) with row stride ldo. */
+ * dx + dc must equal dims[0]; out is (B, dims[n_linear]) with row stride ldo.  The workspace must be 256-byte
+ * aligned on a tensor-core handle (ZK_GEMM_BF16X3 / BF16X1; cudaMalloc and torch allocations are) and 4-byte
+ * aligned on an fp32 one (ZK_EINVAL otherwise). */
 zk_status zk_mlp_forward(const zk_mlp* mlp, const float* x, int64_t ldx, int dx, const float* c,
                          int64_t ldc, int dc, int64_t B, float* out, int64_t ldo, void* workspace,
                          size_t workspace_bytes, zk_stream stream);

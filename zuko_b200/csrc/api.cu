@@ -330,6 +330,11 @@ zk_status zk_mlp_forward(const zk_mlp* m, const float* x, int64_t ldx, int dx, c
     if (B == 0) return ZK_OK;
     ZK_REQUIRE(ws_bytes >= zk_mlp_workspace_bytes(m, B), "mlp_forward: workspace too small (%zu < %zu)",
                ws_bytes, zk_mlp_workspace_bytes(m, B));
+    // the tensor-core path carves its bf16 planes in 256-byte granules, writes them with 16-byte stores and
+    // reads them through 128B-swizzled TMA boxes, which faulted on a workspace based 16 bytes off; the fp32
+    // path keeps floats there.  Refused before anything is launched.
+    const uintptr_t ws_align = (m->gemm_mode != ZK_GEMM_FP32) ? 256 : 4;
+    ZK_REQUIRE((uintptr_t)ws % ws_align == 0, "mlp_forward: workspace must be %d-byte aligned", (int)ws_align);
     cudaStream_t st = (cudaStream_t)stream;
     if (m->gemm_mode != ZK_GEMM_FP32)
         return tc_forward(m, x, ldx, dx, c, ldc, dc, B, out, ldo, ws, ws_bytes, st);
