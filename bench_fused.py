@@ -3,9 +3,9 @@ in one launch) at the shapes of the benchmarked configurations.  Prints one JSON
 
 * ``layers``: per shape and GEMM mode, ms per launch from CUDA events over ``--launches`` launches after warm-up
   (inputs rotate over buffers larger than the 50 MB L2), the kernel's row tile, and the rates the kernel achieves:
-  issued tensor TFLOP/s (every non-zero 64 x 64 weight tile, all split-bf16 terms, over whole row tiles) and
-  weight-streaming GB/s (L2 -> shared memory: each row tile loads every non-zero tile, 16 KB in bf16x3 and 8 KB in
-  bf16x1).  The shapes are the flagship layer (NSF(16, 8, bins=8, hidden=[256] * 3), 2^20 rows) at bf16x3 and at
+  issued tensor TFLOP/s (every non-zero weight tile at the width and depth the kernel multiplies it, all split-bf16
+  terms, over whole row tiles) and weight-streaming GB/s (L2 -> shared memory: each row tile loads every non-zero tile,
+  16 KB in bf16x3 and 8 KB in bf16x1, three quarters of that for an RQS output tile; `zk_layer_fused_stream_bytes`).  The shapes are the flagship layer (NSF(16, 8, bins=8, hidden=[256] * 3), 2^20 rows) at bf16x3 and at
   bf16x1 — half the weight bytes and a third of the MMAs, so the ratio of the two times shows which resource the
   kernel is sensitive to — and the layers of cfg3 (MAF(32, hidden=[512] * 4), 2^20 rows) and cfg5 (NSF(64, 16,
   bins=16, hidden=[512] * 3), 2^21 rows);
@@ -61,6 +61,14 @@ def tile_rows(handle) -> int:
     return int(lib.zk_layer_fused_tile_rows(handle))
 
 
+def stream_bytes(handle, n_tiles: int, gemm_mode: str) -> int:
+    """Weight bytes brought into shared memory per row tile."""
+    lib = E.lib()
+    if not hasattr(lib, "zk_layer_fused_stream_bytes"):  # libraries older than the query stream whole 64 x 64 tiles
+        return n_tiles * (16384 if gemm_mode == "bf16x3" else 8192)
+    return int(lib.zk_layer_fused_stream_bytes(handle))
+
+
 def time_layer(s, dev, args, clk_rows: list) -> dict:
     layer = build_layer(s, dev)
     B, D, C = s["rows"], s["D"], s["C"]
@@ -95,12 +103,12 @@ def time_layer(s, dev, args, clk_rows: list) -> dict:
     ms = e0.elapsed_time(e1) / args.launches
     n_tiles, issued_macs_per_row = int(info[1]), info[2]
     row_tiles = math.ceil(B / rows)
-    tile_bytes = 16384 if s["gemm_mode"] == "bf16x3" else 8192
+    tile_stream = stream_bytes(handle, n_tiles, s["gemm_mode"])
     return {
         "name": s["name"], "gemm_mode": s["gemm_mode"], "rows": B, "tile_rows": rows, "weight_tiles_per_row_tile": n_tiles,
         "ms_per_launch": ms, "launches": args.launches,
         "issued_tflops": 2.0 * issued_macs_per_row * row_tiles * rows / (ms * 1e-3) / 1e12,
-        "weight_stream_gbs": row_tiles * n_tiles * tile_bytes / (ms * 1e-3) / 1e9,
+        "weight_stream_gbs": row_tiles * tile_stream / (ms * 1e-3) / 1e9,
     }  # fmt: skip
 
 

@@ -273,8 +273,13 @@ size_t zk_layer_workspace_bytes(const zk_layer* layer, int64_t B);
  * 207-215) and how much tensor-core work it issues.  Returns 0 = per-layer GEMM kernels,
  * 1 = fused layer kernel; out[0] = the same,
  * out[1] = non-zero 64 x 64 weight tiles per row tile, out[2] = MACs ISSUED per sample row (non-zero tiles only, all
- * split-bf16 terms), out[3] = dense MACs per sample row (what nn.py:218 executes). */
+ * split-bf16 terms; an output-layer tile is multiplied at the width of its parameter rows, 48 for RQS, and layer 0's
+ * last K block over the 16-wide steps that hold inputs), out[3] = dense MACs per sample row (what nn.py:218
+ * executes). */
 int zk_layer_fused_info(const zk_layer* layer, double* out);
+/* Weight bytes the fused layer kernel brings into shared memory per row tile (the tiles of out[1], all bf16 planes
+ * of the GEMM mode: 64 x 64 boxes, 48 x 64 for the output layer of RQS); 0 when the layer does not run fused. */
+size_t zk_layer_fused_stream_bytes(const zk_layer* layer);
 /* Rows per tile of the fused layer kernel for this layer, chosen from its shape: 128 (two consumer warpgroups
  * share every streamed weight tile), 64, or 0 when the layer does not run as the fused kernel.  Read-only. */
 int zk_layer_fused_tile_rows(const zk_layer* layer);

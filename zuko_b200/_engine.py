@@ -138,6 +138,7 @@ _SIGNATURES = {
     "zk_layer_workspace_bytes": (c_size_t, [_P, c_int64]),
     "zk_layer_fused_info": (c_int, [_P, c_void_p]),
     "zk_layer_fused_tile_rows": (c_int, [_P]),
+    "zk_layer_fused_stream_bytes": (c_size_t, [_P]),
     "zk_layer_fused_plan": (c_int, [_P, POINTER(c_int), POINTER(c_size_t)]),
     "zk_layer_inverse_geometry": (c_int, [_P, POINTER(c_int), POINTER(c_int), POINTER(c_size_t)]),
     "zk_layer_sequential_inverse": (c_int, [_P]),

@@ -567,6 +567,12 @@ int zk_layer_fused_info(const zk_layer* l, double* out) {
     return kind;
 }
 
+size_t zk_layer_fused_stream_bytes(const zk_layer* l) {
+    double info[4];
+    if (zk_layer_fused_info(l, info) != 1) return 0;
+    return tc_pack_of(l->hyper)->fused.stream_bytes;
+}
+
 int zk_layer_fused_tile_rows(const zk_layer* l) {
     if (!l || l->kind != ZK_LAYER_AUTOREGRESSIVE || !l->hyper || l->circ) return 0;
     return fused_tile_rows(l->hyper, l->uni, l->K, l->D, l->C);

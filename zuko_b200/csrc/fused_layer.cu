@@ -3,7 +3,8 @@
 //   x, c  --(bf16 hi/lo split, in-kernel)-->  A operand in SHARED MEMORY (64 or 128 rows x up to 512 columns)
 //   for every linear layer:  wgmma  D[registers] += A[smem] * W[smem]^T
 //        W is streamed from L2 by TMA as 64 x 64 tiles (hi + lo planes) through a ring of mbarrier
-//        slots; the all-zero tiles of the degree-sorted masked matrices are never loaded or multiplied;
+//        slots; the all-zero tiles of the degree-sorted masked matrices are never loaded or multiplied,
+//        nor are the k16 steps of layer 0 past D + C or the padding rows of an output chunk past NL;
 //        hidden layers : at most four 64 x 64 fp32 accumulators per consumer warpgroup; once every
 //                        reader of an A operand is done with it, it is overwritten in place with the
 //                        layer's output (bias, activation, bf16 hi/lo split): activations never
@@ -68,6 +69,9 @@ struct FusedParams {
     uint8_t kbmask[ZK_FUSED_MAX_LINEAR][128];  // [layer][chunk]: K blocks with non-zero weights
     int n_linear;
     int K0, KB0;        // real input width (D + C) and its number of 64-wide K blocks
+    int ks0;            // k16 steps of layer 0's last K block that hold inputs: ceil((K0 - 64 (KB0 - 1)) / 16)
+    int vec_in;         // x and c rows can be read as float4 (D, C, ldx, ldc multiples of 4, 16-byte aligned bases)
+    int g_shift;        // vec_in: log2 of the staging items per row (float4 groups of the staged columns, rounded up)
     int H;              // hidden width (multiple of 64, <= 512)
     int KBA;            // K blocks of the A buffer: max(KB0, H / 64)
     int D, C;
@@ -84,17 +88,33 @@ struct FusedParams {
     float bound, aw, ad;
 };
 
-// one 64 x 64 tile of the current layer: A K block kb times the W tile in ring slot `w_tile`,
-// into accumulator q (compile-time index: the accumulators must stay in registers)
-__device__ __forceinline__ void tile_mma(float (&acc)[4][32], int q, uint32_t a_hi, uint32_t a_plane, uint32_t w_tile,
-                                         int n_terms) {
+// f(integral_constant<int, ks>), ks in 1..4: the k16 steps of an MMA chain are a compile-time constant, chosen by
+// one branch outside the chain
+template <class F>
+__device__ __forceinline__ void with_ksteps(int ks, F&& f) {
+    if (ks == 4) f(std::integral_constant<int, 4>{});
+    else if (ks == 3) f(std::integral_constant<int, 3>{});
+    else if (ks == 2) f(std::integral_constant<int, 2>{});
+    else f(std::integral_constant<int, 1>{});
+}
+
+// one synchronous 64 x N tile: the first KS k16 steps of an A K block times the W tile in ring slot `w_tile`
+template <int KS = 4, int NA>
+__device__ __forceinline__ void tile_mma(float (&acc)[NA], uint32_t a_hi, uint32_t a_plane, uint32_t w_tile, int n_terms) {
     wgmma_fence();
-    if (q == 0) wgmma_kblock(acc[0], a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
-    else if (q == 1) wgmma_kblock(acc[1], a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
-    else if (q == 2) wgmma_kblock(acc[2], a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
-    else wgmma_kblock(acc[3], a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
+    wgmma_kblock<KS>(acc, a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
     wgmma_commit();
     wgmma_wait0();
+    acc_fence(acc);
+}
+// the same into accumulator q of a hidden layer (compile-time index: the accumulators must stay in registers)
+template <int KS>
+__device__ __forceinline__ void tile_mma(float (&acc)[4][32], int q, uint32_t a_hi, uint32_t a_plane, uint32_t w_tile,
+                                         int n_terms) {
+    if (q == 0) tile_mma<KS>(acc[0], a_hi, a_plane, w_tile, n_terms);
+    else if (q == 1) tile_mma<KS>(acc[1], a_hi, a_plane, w_tile, n_terms);
+    else if (q == 2) tile_mma<KS>(acc[2], a_hi, a_plane, w_tile, n_terms);
+    else tile_mma<KS>(acc[3], a_hi, a_plane, w_tile, n_terms);
 #pragma unroll
     for (int i = 0; i < 4; ++i) acc_fence(acc[i]);
 }
@@ -105,10 +125,10 @@ template <int UNI, int KT, bool FAST, bool GACT, int ROWS, int NT>
 __global__ void __launch_bounds__(F_THREADS, 1)
 fused_layer_kernel(const __grid_constant__ FusedParams p) {
     using Cfg = LastCfg<UNI, KT>;
-    constexpr int P = Cfg::P, DPC = Cfg::DPC;
+    constexpr int P = Cfg::P, DPC = Cfg::DPC, NL = Cfg::NL;
     constexpr int NP = DPC * P, SROW = f_srow(NP);  // staged columns of an output chunk, staging row stride
     constexpr bool WIDE = (ROWS == 128);
-    static_assert(NP <= FK, "a last-layer chunk must fit 64 columns");
+    static_assert(NP <= NL && NL <= FK && NL % 8 == 0, "a last-layer chunk must fit its MMA width");
     static_assert(ROWS == 64 || ROWS == 128, "row tile: one or two wgmma M");
     const int n_terms = NT ? NT : p.n_terms;
 
@@ -143,14 +163,14 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
         // its chunks; the output layer chunk by chunk, each over its K blocks
         if constexpr (WIDE) setmaxnreg_dec<40>();
         if (threadIdx.x == 0) {
-            const uint32_t bytes = (n_terms == 3) ? F_STAGE : F_TILE;
             int rs[2] = {0, 0};
             uint32_t rph[2] = {0u, 0u};
-            auto load = [&](int l, int ch, int kb) {  // 64 rows: chunk ch is multiplied by consumer warpgroup ch % 2
+            // 64 rows: chunk ch is multiplied by consumer warpgroup ch % 2.  plane: bytes of the layer's box
+            auto load = [&](int l, int ch, int kb, uint32_t plane) {
                 const int o = WIDE ? 0 : (ch & 1), s = o * NR + rs[o];
                 mbar_wait(&empty[s], rph[o] ^ 1);
                 uint8_t* dst = sW + (size_t)s * F_STAGE;
-                mbar_arrive_expect_tx(&full[s], bytes);
+                mbar_arrive_expect_tx(&full[s], (n_terms == 3) ? 2 * plane : plane);
                 tma_load_3d(dst, &p.mapW[l], &full[s], kb * FK, ch * FK, 0);
                 if (n_terms == 3) tma_load_3d(dst + F_TILE, &p.mapW[l], &full[s], kb * FK, ch * FK, 1);
                 if (++rs[o] == NR) { rs[o] = 0; rph[o] ^= 1; }
@@ -160,11 +180,11 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                     const int KB = (l == 0) ? p.KB0 : nch;
                     for (int kb = 0; kb < KB; ++kb)
                         for (int ch = 0; ch < nch; ++ch)
-                            if ((p.kbmask[l][ch] >> kb) & 1u) load(l, ch, kb);
+                            if ((p.kbmask[l][ch] >> kb) & 1u) load(l, ch, kb, F_TILE);
                 }
                 for (int ch = 0; ch < p.n_last; ++ch)
                     for (int kb = 0; kb < nch; ++kb)
-                        if ((p.kbmask[L - 1][ch] >> kb) & 1u) load(L - 1, ch, kb);
+                        if ((p.kbmask[L - 1][ch] >> kb) & 1u) load(L - 1, ch, kb, NL * FK * 2);
             }
         }
         return;
@@ -191,9 +211,37 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
         const int64_t rb = (int64_t)t * ROWS + (WIDE ? cw * FM : 0);  // first row of this warpgroup's A
         if constexpr (!WIDE) named_bar_sync(1, 256);  // the previous tile's MMAs on A and reads of s_part are done
         // ---- stage the layer-0 operand: cat(x, c) -> bf16 hi / lo pairs, 128B-swizzled K blocks ----
-        {
-            const int kw = p.KB0 * (FK / 2);  // bf16 pairs per row
-            const int n_thr = WIDE ? 128 : 256;
+        // Only the columns layer 0 multiplies are written (zeros from K0 on); what lies beyond in the last K block
+        // is the previous tile's activations, which layer 0 does not read and the first epilogue overwrites.
+        const int KW = (p.KB0 - 1) * FK + 16 * p.ks0;
+        const int n_thr = WIDE ? 128 : 256;
+        if (p.vec_in) {
+            // item i = (row i >> g_shift, float4 group i & mask); four loads in flight per thread before the first split
+            const int n_it = FM << p.g_shift, gmask = (1 << p.g_shift) - 1;
+            for (int i0 = WIDE ? tid : ctid; i0 < n_it; i0 += 4 * n_thr) {
+                float4 v[4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int i = i0 + j * n_thr, k = (i & gmask) << 2;
+                    const int64_t row = rb + (i >> p.g_shift);
+                    v[j] = make_float4(0.f, 0.f, 0.f, 0.f);  // masked rows and padded columns stage zeros
+                    const float* src = (k < p.D) ? p.x + row * p.ldx + k : p.c + row * p.ldc + (k - p.D);
+                    if (i < n_it && row < p.M && k < p.K0) v[j] = __ldg(reinterpret_cast<const float4*>(src));
+                }
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int i = i0 + j * n_thr, k = (i & gmask) << 2;
+                    if (i >= n_it || k >= KW) continue;
+                    uint2 hi, lo;
+                    split2_bf16(v[j].x, v[j].y, hi.x, lo.x);
+                    split2_bf16(v[j].z, v[j].w, hi.y, lo.y);
+                    const uint32_t off = (uint32_t)(k >> 6) * F_TILE + sw128_offset(i >> p.g_shift, k & 63);
+                    *reinterpret_cast<uint2*>(myA + off) = hi;
+                    *reinterpret_cast<uint2*>(myA + a_plane + off) = lo;
+                }
+            }
+        } else {
+            const int kw = KW / 2;  // bf16 pairs per row
             for (int i = WIDE ? tid : ctid; i < FM * kw; i += n_thr) {
                 const int r = i / kw, k = 2 * (i - r * kw);
                 const int64_t row = rb + r;
@@ -226,14 +274,17 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                 // accumulator q = chunk q; one group per tile, its slot released once the next tile is issued
                 int held = -1;
                 for (int kb = 0; kb < KB; ++kb) {
+                    const int ks = (l == 0 && kb == KB - 1) ? p.ks0 : 4;
 #pragma unroll
                     for (int q = 0; q < F_WIDE_MAXKB; ++q) {
                         if (q >= nch || !((p.kbmask[l][q] >> kb) & 1u)) continue;
                         mbar_wait(&full[s], ph);
                         const uint32_t a_hi = a_base + (uint32_t)kb * F_TILE, w_tile = w_base + (uint32_t)s * F_STAGE;
-                        wgmma_fence();
-                        wgmma_kblock(acc[q], a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
-                        wgmma_commit();
+                        with_ksteps(ks, [&](auto KS) {
+                            wgmma_fence();
+                            wgmma_kblock<decltype(KS)::value>(acc[q], a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
+                            wgmma_commit();
+                        });
                         wgmma_wait1();
                         if (held >= 0) release(held);
                         held = s;
@@ -246,11 +297,15 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                 for (int q = 0; q < 4; ++q) acc_fence(acc[q]);
             } else {
                 for (int kb = 0; kb < KB; ++kb) {
+                    const int ks = (l == 0 && kb == KB - 1) ? p.ks0 : 4;
                     for (int ch = 0; ch < nch; ++ch) {
                         if (!((p.kbmask[l][ch] >> kb) & 1u)) continue;
                         if ((ch & 1) == cw) {
                             mbar_wait(&full[s], ph);
-                            tile_mma(acc, ch >> 1, a_base + (uint32_t)kb * F_TILE, a_plane, w_base + (uint32_t)s * F_STAGE, n_terms);
+                            with_ksteps(ks, [&](auto KS) {
+                                tile_mma<decltype(KS)::value>(acc, ch >> 1, a_base + (uint32_t)kb * F_TILE, a_plane,
+                                                              w_base + (uint32_t)s * F_STAGE, n_terms);
+                            });
                             release(s);
                             advance();
                         }
@@ -295,9 +350,9 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
         const bool row_ok = row < p.M;
         const float* bias = p.bias[L - 1];
         // accumulators (+ bias) of output chunk ch -> this warpgroup's staging buffer
-        auto stage_chunk = [&](const float (&a)[32], int ch) {
+        auto stage_chunk = [&](const float (&a)[NL / 2], int ch) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
+            for (int i = 0; i < NL / 8; ++i) {
                 if (8 * i >= NP) break;
                 const int col = 8 * i + 2 * (lane & 3);
                 const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + ch * FK + col));
@@ -362,11 +417,11 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
             // a chunk's tiles (at most F_WIDE_MAXKB <= n_stages) are multiplied as one batch of asynchronous MMAs and
             // released together once they are done.  The bijector runs with no MMAs in flight: its divergent
             // branches inside a wgmma pipeline stage make ptxas serialize every wgmma of the kernel (C7515).
-            float acc[32];
+            float acc[NL / 2];
             float ls0 = 0.f, ls1 = 0.f;  // partials of the even and of the odd chunks
             auto out_chunk = [&](int ch, float& ls) {
 #pragma unroll
-                for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+                for (int i = 0; i < NL / 2; ++i) acc[i] = 0.f;
                 const int hs = s;
                 int hn = 0;
                 for (int kb = 0; kb < nch; ++kb) {
@@ -397,20 +452,20 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
             float lsum = 0.f;
             for (int ch = 0; ch < p.n_last; ++ch) {
                 const bool mine = (ch & 1) == cw;
-                float acc[4][32];
+                float acc[NL / 2];
 #pragma unroll
-                for (int i = 0; i < 32; ++i) acc[0][i] = 0.f;
+                for (int i = 0; i < NL / 2; ++i) acc[i] = 0.f;
                 for (int kb = 0; kb < nch; ++kb) {
                     if (!((p.kbmask[L - 1][ch] >> kb) & 1u)) continue;
                     if (mine) {
                         mbar_wait(&full[s], ph);
-                        tile_mma(acc, 0, a_base + (uint32_t)kb * F_TILE, a_plane, w_base + (uint32_t)s * F_STAGE, n_terms);
+                        tile_mma(acc, a_base + (uint32_t)kb * F_TILE, a_plane, w_base + (uint32_t)s * F_STAGE, n_terms);
                         release(s);
                         advance();
                     }
                 }
                 if (!mine) continue;
-                stage_chunk(acc[0], ch);
+                stage_chunk(acc, ch);
                 named_bar_sync(2 + cw, 128);
                 eval_chunk(ch, lsum);
                 named_bar_sync(2 + cw, 128);  // staging buffer free for the next chunk
@@ -504,6 +559,9 @@ int fused_layer_kind(const zk_mlp* m, int univariate, int bins, int D, int C) {
 }
 
 // K blocks of the fused kernel's A operand: the wider of the input and the hidden width
+// k16 steps of layer 0's last K block that hold inputs
+static int fused_ks0(int K0, int KB0) { return (K0 - FK * (KB0 - 1) + 15) / 16; }
+
 static int fused_kba(const zk_mlp* m) {
     return std::max(((const TcPack*)m->tc)->layers[0].Kp / FK, m->dims[1] / FK);
 }
@@ -658,11 +716,17 @@ zk_status fused_layer_prepare(zk_mlp* m, const uint8_t* const* mask_dev, int uni
     }
     ZK_TRY(fused_split(m, f, 0));
     ZK_CUDA(cudaStreamSynchronize(0));
-    f.map64.assign(L, CUtensorMap{});
-    for (int l = 0; l < L; ++l) ZK_TRY(make_plane_map(&f.map64[l], f.w[l], fused_rows(m, f, l), pk->layers[l].Kp, 64));
+    // the output layer's box covers the NL rows of a 64-row chunk that hold parameters
+    const int NL = fused_nl(univariate, bins);
+    f.maps.assign(L, CUtensorMap{});
+    for (int l = 0; l < L; ++l)
+        ZK_TRY(make_plane_map(&f.maps[l], f.w[l], fused_rows(m, f, l), pk->layers[l].Kp, l == L - 1 ? NL : FK));
     // ---- which (chunk, K block) tiles of the permuted masked matrices are non-zero ----
     memset(f.kbmask, 0, sizeof(f.kbmask));
     f.n_items = 0;
+    f.issued_macs_per_row = 0;
+    f.stream_bytes = 0;
+    const int KB0 = pk->layers[0].Kp / FK, planes = (pk->n_terms == 3) ? 2 : 1;
     for (int l = 0; l < L; ++l) {
         const bool last = (l == L - 1);
         const int K = m->dims[l];
@@ -679,9 +743,17 @@ zk_status fused_layer_prepare(zk_mlp* m, const uint8_t* const* mask_dev, int uni
             }
             f.kbmask[l][ch] = bits;
             f.n_items += __builtin_popcount(bits);
+            // what the kernel issues and streams for these tiles: N = NL in the output layer, fused_ks0 k16 steps in
+            // layer 0's last K block (whose box is still 64 columns wide)
+            const int n = last ? NL : FK;
+            for (int kb = 0; kb < 8; ++kb) {
+                if (!((bits >> kb) & 1)) continue;
+                const int k = (l == 0 && kb == KB0 - 1) ? 16 * fused_ks0(m->dims[0], KB0) : FK;
+                f.issued_macs_per_row += (double)n * k * pk->n_terms;
+                f.stream_bytes += (size_t)n * FK * 2 * planes;
+            }
         }
     }
-    f.issued_macs_per_row = (double)f.n_items * FK * FK * pk->n_terms;  // every tile is 64 x 64 MACs per row
     f.uni = univariate; f.bins = bins; f.D = D; f.C = C;
     f.ready = true;
     return ZK_OK;
@@ -697,12 +769,16 @@ zk_status launch_fused_layer(const zk_mlp* m, const FusedLayerArgs& a, cudaStrea
     memset(&p, 0, sizeof(p));
     memcpy(p.kbmask, f.kbmask, sizeof(p.kbmask));
     for (int i = 0; i < m->n_linear; ++i) {
-        p.mapW[i] = f.map64[i];
+        p.mapW[i] = f.maps[i];
         p.bias[i] = f.bias[i];
     }
     p.n_linear = m->n_linear;
     p.K0 = a.D + a.C;
     p.KB0 = pk->layers[0].Kp / FK;
+    p.ks0 = fused_ks0(p.K0, p.KB0);
+    const auto vec4 = [](const float* q, int n, int64_t ld) { return n % 4 == 0 && ld % 4 == 0 && ((uintptr_t)q & 15) == 0; };
+    p.vec_in = vec4(a.x, a.D, a.ldx) && (a.C == 0 || vec4(a.c, a.C, a.ldc));
+    while ((4 << p.g_shift) < (p.KB0 - 1) * FK + 16 * p.ks0) ++p.g_shift;
     p.H = m->dims[1];
     p.KBA = fused_kba(m);
     p.D = a.D; p.C = a.C;

@@ -58,9 +58,10 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
-__device__ __forceinline__ void acc_fence(float (&d)[32]) {
+template <int NA>
+__device__ __forceinline__ void acc_fence(float (&d)[NA]) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+    for (int i = 0; i < NA; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // D[64 x 64] += A[64 x 16] * B[64 x 16]^T (one warpgroup; bf16 inputs, fp32 accumulators in registers).
@@ -83,22 +84,46 @@ __device__ __forceinline__ void wgmma_m64n64k16_bf16(float (&d)[32], uint64_t de
         : "l"(desc_a), "l"(desc_b));
 }
 
-// One 64-wide K block of the split-bf16 product on 64 x 64 tiles: hi*hi (+ hi*lo + lo*hi when n_terms == 3).
+// D[64 x 48] += A[64 x 16] * B[48 x 16]^T: the first 48 rows (six 8-row groups) of a 64-row B tile, same descriptor.
+// Accumulator layout as above with i < 6.
+__device__ __forceinline__ void wgmma_m64n48k16_bf16(float (&d)[24], uint64_t desc_a, uint64_t desc_b) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23}, "
+        "%24, %25, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "l"(desc_a), "l"(desc_b));
+}
+// one k16 step on an accumulator of N / 2 registers per thread, N = 64 or 48
+__device__ __forceinline__ void wgmma_k16(float (&d)[32], uint64_t a, uint64_t b) { wgmma_m64n64k16_bf16(d, a, b); }
+__device__ __forceinline__ void wgmma_k16(float (&d)[24], uint64_t a, uint64_t b) { wgmma_m64n48k16_bf16(d, a, b); }
+
+// The first KS 16-wide k steps of one 64-wide K block of the split-bf16 product on 64 x N tiles (N = 2 NA): hi*hi
+// (+ hi*lo + lo*hi when n_terms == 3).  KS < 4 when the columns past 16 KS of the A operand are padding.
 // a_hi / a_lo / b_hi / b_lo: shared-memory addresses of 128B-swizzled K-major 64-row operand tiles.
-__device__ __forceinline__ void wgmma_kblock(float (&d)[32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+template <int KS = 4, int NA>
+__device__ __forceinline__ void wgmma_kblock(float (&d)[NA], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
                                              int n_terms) {
+    static_assert(KS >= 1 && KS <= 4, "a K block is four k16 steps");
     const uint64_t dah = gmma_desc_sw128(a_hi), dal = gmma_desc_sw128(a_lo);
     const uint64_t dbh = gmma_desc_sw128(b_hi), dbl = gmma_desc_sw128(b_lo);
     if (n_terms == 3) {  // one branch outside the MMA sequence: no register hand-off between the MMAs
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            wgmma_m64n64k16_bf16(d, gmma_desc_advance(dah, k), gmma_desc_advance(dbh, k));
-            wgmma_m64n64k16_bf16(d, gmma_desc_advance(dah, k), gmma_desc_advance(dbl, k));
-            wgmma_m64n64k16_bf16(d, gmma_desc_advance(dal, k), gmma_desc_advance(dbh, k));
+        for (int k = 0; k < KS; ++k) {
+            wgmma_k16(d, gmma_desc_advance(dah, k), gmma_desc_advance(dbh, k));
+            wgmma_k16(d, gmma_desc_advance(dah, k), gmma_desc_advance(dbl, k));
+            wgmma_k16(d, gmma_desc_advance(dal, k), gmma_desc_advance(dbh, k));
         }
     } else {
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_m64n64k16_bf16(d, gmma_desc_advance(dah, k), gmma_desc_advance(dbh, k));
+        for (int k = 0; k < KS; ++k) wgmma_k16(d, gmma_desc_advance(dah, k), gmma_desc_advance(dbh, k));
     }
 }
 
@@ -124,10 +149,11 @@ struct FusedPack {
     std::vector<int*> dperm;        // per hidden layer: device copy of the degree permutation (owned; weight refresh)
     int* last_rows = nullptr;       // device: output-layer row of every padded output row, -1 = zero row (owned)
     int n_last = 0;                 // 64-row chunks of the output layer
-    std::vector<CUtensorMap> map64; // box (64 x 64 x 1)
+    std::vector<CUtensorMap> maps;  // box (64 x 64 x 1); output layer (64 x NL x 1): a chunk's parameter rows
     uint8_t kbmask[8][128];         // [layer][chunk]: bit kb = K block kb has non-zero weights
     double issued_macs_per_row = 0;  // MACs the kernel issues per sample row (all split terms), bench bookkeeping
     int n_items = 0;                 // non-zero 64 x 64 weight tiles streamed per row tile
+    size_t stream_bytes = 0;         // weight bytes those tiles bring into shared memory per row tile (all planes)
 };
 struct TcPack {
     std::vector<TcLayer> layers;
