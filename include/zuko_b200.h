@@ -385,10 +385,20 @@ typedef struct {
 
 /* d/d(x, phi) of MonotonicRQSTransform(*phi).call_and_ladj(x) (transforms.py:469-567) for upstream
  * gradients grad_y (B, D) and grad_ladj (B, of the per-sample summed ladj); either may be NULL (= 0).
- * grad_phi: (B, D*P) per-sample gradients when phi_ld != 0 (may alias phi when phi_ld == D*P), or the
- * (D, P) table gradient, ACCUMULATED, when phi_ld == 0.  grad_x / grad_phi may be NULL.
+ * grad_phi: (B, D*P) per-sample gradients when phi_ld != 0, or the (D, P) table gradient, ACCUMULATED,
+ * when phi_ld == 0.  grad_phi must not overlap phi, except grad_phi == phi with phi_ld == D*P (the
+ * gradients overwrite the parameters); any other overlap, a shared table included, returns ZK_EINVAL
+ * before anything runs.  grad_x / grad_phi may be NULL.
  * workspace >= zk_univariate_backward_workspace_bytes(B, D, P, phi_ld). */
 size_t zk_univariate_backward_workspace_bytes(int64_t B, int D, int P, int64_t phi_ld);
+/* Tile plan of the bijector backward kernel for these arguments (as zk_univariate_plan for the forward): returns ZK_OK
+ * and fills the non-NULL outputs, or the status the launch would return for this shape.  rows_per_tile: sample rows
+ * per CTA; smem: dynamic shared memory bytes (R parameter rows, plus a shared table beside them when R > 1; at R = 1
+ * the table is rewritten in place, so one row of up to 200 KB fits either way); instantiated: the compile-time shape
+ * (RQS 8 or 16, Gaussianization 8 or 16, SOSP 3 for (K, degree) = (3, 4), Bernstein 17 for degree 16; 0 for the
+ * runtime-shape and affine kernels).  B = 0 reports 0 everywhere.  Read-only, no device work. */
+zk_status zk_univariate_backward_plan(int univariate, int64_t B, int D, int K, int degree, int64_t phi_ld,
+                                      int* rows_per_tile, size_t* smem, int* instantiated);
 zk_status zk_rqs_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
                           int D, int K, float bound, float slope, const float* grad_y, int64_t ldgy,
                           const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi,

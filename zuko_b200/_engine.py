@@ -160,6 +160,8 @@ _SIGNATURES = {
     "zk_flow_log_prob": (c_int, [POINTER(FlowDesc), _P, c_int64, _P, c_int64, c_int64, _P, _P, _P, c_size_t, _P]),
     "zk_flow_inverse": (c_int, [POINTER(FlowDesc), _P, c_int64, _P, c_int64, c_int64, _P, c_int64, _P, _P, c_size_t, _P]),
     "zk_univariate_backward_workspace_bytes": (c_size_t, [c_int64, c_int, c_int, c_int64]),
+    "zk_univariate_backward_plan": (c_int, [c_int, c_int64, c_int, c_int, c_int, c_int64, POINTER(c_int), POINTER(c_size_t),
+                                            POINTER(c_int)]),
     "zk_rqs_backward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, c_float, c_float, _P, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),
     "zk_affine_backward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_float, _P, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),
     "zk_gaussianization_backward": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int, c_int, _P, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),

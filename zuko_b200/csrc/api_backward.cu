@@ -614,6 +614,16 @@ zk_status uni_backward_entry(int uni, const float* x, int64_t ldx, const float* 
                              void* ws, size_t ws_bytes, cudaStream_t st, int degree = 0, float eps = kBernsteinEps) {
     ZK_REQUIRE(x && phi && B >= 0 && D > 0, "univariate backward: bad arguments");
     const int P = uni_param_count(uni, K, degree);
+    if (gphi != nullptr && B > 0 && P > 0) {
+        // grad_phi may only be phi itself with dense rows: each tile then rewrites the rows it staged.  Any
+        // other overlap lets one CTA's (or one chunk's) writes reach parameters another one still reads
+        const int64_t DP = (int64_t)D * P;
+        const int64_t n_phi = (phi_ld == 0) ? DP : (B - 1) * phi_ld + DP;
+        const int64_t n_gphi = (phi_ld == 0) ? DP : B * DP;
+        const bool overlap = (uintptr_t)gphi < (uintptr_t)(phi + n_phi) && (uintptr_t)phi < (uintptr_t)(gphi + n_gphi);
+        ZK_REQUIRE(!overlap || (gphi == phi && phi_ld == DP),
+                   "univariate backward: grad_phi overlaps phi (only grad_phi == phi with phi_ld == D*P is allowed)");
+    }
     UniBwdArgs u;
     u.univariate = uni; u.K = K; u.degree = degree; u.bound = bound; u.slope = slope; u.eps = eps; u.D = D;
     u.fast_math = g_fast_math.load() != 0;
@@ -644,6 +654,16 @@ zk_status uni_backward_entry(int uni, const float* x, int64_t ldx, const float* 
 extern "C" {
 
 int zk_set_tc_backward(int on) { return g_tc_backward.exchange(on ? 1 : 0); }
+
+zk_status zk_univariate_backward_plan(int univariate, int64_t B, int D, int K, int degree, int64_t phi_ld,
+                                      int* rows_per_tile, size_t* smem, int* instantiated) {
+    UniBwdPlan p;
+    ZK_TRY(uni_bwd_plan(univariate, B, D, K, degree, phi_ld, p));
+    if (rows_per_tile) *rows_per_tile = p.rows_per_tile;
+    if (smem) *smem = p.smem;
+    if (instantiated) *instantiated = p.kt;
+    return ZK_OK;
+}
 
 size_t zk_univariate_backward_workspace_bytes(int64_t B, int D, int P, int64_t phi_ld) {
     if (phi_ld != 0 || B <= 0 || D <= 0 || P <= 0) return 0;

@@ -56,6 +56,8 @@ __device__ __forceinline__ float circ_shift_b(float x, float bound) {  // biject
 // thread = (sample row, dim) pair; the tile's parameter block is staged in shared memory, every
 // pair rewrites its P slots with the parameter gradients, and the tile is written back with
 // coalesced stores (per-sample gradients (B, D*P); a shared table is reduced by the caller).
+// A shared table is rewritten in place too when the tile holds one row (uni_bwd_plan): pair d then
+// reads and writes only slots d*P.., and every CTA stages its own copy of the table.
 template <int UNI, int KT, bool FAST>
 __global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const typename BwdParamsFor<UNI>::type a) {
     extern __shared__ __align__(16) float smem[];
@@ -66,7 +68,7 @@ __global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const typename Bwd
     const int npairs = nrows * D;
     const bool shared_tbl = (a.phi_ld == 0);
     float* s_phi = smem;
-    float* s_out = shared_tbl ? smem + D * P : smem;  // in place unless the table is shared
+    float* s_out = (shared_tbl && a.rows_per_tile > 1) ? smem + D * P : smem;
     const int n_phi = shared_tbl ? D * P : npairs * P;
     if (shared_tbl) {
         for (int i = tid; i < n_phi; i += kBwdThreads) s_phi[i] = a.phi[i];
@@ -334,9 +336,10 @@ int wgrad_slices_max(int N, int K) {
 }
 
 template <int UNI, int KT>
-zk_status launch_uni_bwd_t(const typename BwdParamsFor<UNI>::type& p, bool fast, int grid, size_t smem, cudaStream_t st) {
+zk_status launch_uni_bwd_t(const typename BwdParamsFor<UNI>::type& p, bool fast, int grid, size_t smem, bool smem_attr,
+                           cudaStream_t st) {
     auto go = [&](auto kern) -> zk_status {
-        if (smem > 40 * 1024)
+        if (smem_attr)
             ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, kBwdThreads, smem, st>>>(p);
         return check_launch("uni_bwd_kernel");
@@ -349,29 +352,64 @@ zk_status launch_uni_bwd_t(const typename BwdParamsFor<UNI>::type& p, bool fast,
 
 }  // namespace
 
+zk_status uni_bwd_plan(int uni, int64_t B, int D, int K, int degree, int64_t phi_ld, UniBwdPlan& out) {
+    ZK_REQUIRE(B >= 0 && D > 0, "univariate backward: bad shape B=%lld D=%d", (long long)B, D);
+    out = UniBwdPlan{};
+    if (B == 0) return ZK_OK;
+    ZK_REQUIRE(uni == ZK_UNI_AFFINE || uni == ZK_UNI_RQS || uni == ZK_UNI_GAUSS || uni == ZK_UNI_SOSP || uni == ZK_UNI_BERNSTEIN,
+               "univariate backward: unknown kind %d", uni);
+    if (uni == ZK_UNI_RQS) {
+        ZK_REQUIRE(K >= 1 && K <= 1024, "rqs backward: bins must be in [1, 1024], got %d", K);
+        out.kt = (K == 8 || K == 16) ? K : 0;
+    } else if (uni == ZK_UNI_GAUSS) {
+        ZK_REQUIRE(K >= 1 && K <= 1024, "gaussianization backward: components must be in [1, 1024], got %d", K);
+        out.kt = (K == 8 || K == 16) ? K : 0;
+    } else if (uni == ZK_UNI_SOSP) {
+        ZK_REQUIRE(sosp_shape_ok(K, degree), "sosp backward: polynomials %d / degree %d out of range", K, degree);
+        out.kt = (K == sosp::kDefK && degree == sosp::kDefL) ? sosp::kDefK : 0;
+    } else if (uni == ZK_UNI_BERNSTEIN) {
+        ZK_REQUIRE(bernstein_shape_ok(degree), "bernstein backward: degree must be in [0, 59], got %d", degree);
+        out.kt = (degree + 1 == bern::kDefP) ? bern::kDefP : 0;
+    }
+    const int P = uni_param_count(uni, K, degree);
+    ZK_REQUIRE(phi_ld == 0 || phi_ld >= (int64_t)D * P, "univariate backward: phi_ld too small");
+
+    // tile = R rows: aim at >= 256 pairs and ~24 KB of phi per CTA, at most 96 KB with a shared table staged
+    // beside the rows; one row up to 200 KB (a shared table is then rewritten in place)
+    const size_t row_bytes = (size_t)D * P * 4;
+    const size_t table = (phi_ld == 0) ? row_bytes : 0;
+    ZK_REQUIRE(row_bytes <= 200 * 1024, "univariate backward: D*P too large for one tile (%zu B)", row_bytes);
+    int64_t R = (int64_t)(24 * 1024 / row_bytes);
+    const int64_t r_pairs = ceil_div(kBwdThreads, D);
+    if (R < r_pairs) R = r_pairs;
+    while (R > 1 && R * row_bytes + table > 96 * 1024) --R;
+    if (R < 1) R = 1;
+    if (R > B) R = B;
+    const int64_t grid = ceil_div(B, R);
+    ZK_REQUIRE(grid <= 0x7fffffff, "univariate backward: batch too large for one launch");
+    out.rows_per_tile = (int)R;
+    out.grid = (int)grid;
+    out.table_in_place = (phi_ld == 0 && R == 1);
+    out.smem = (size_t)R * row_bytes + (out.table_in_place ? 0 : table);
+    out.smem_attr = out.smem > 40 * 1024;
+    return ZK_OK;
+}
+
 zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
     ZK_REQUIRE(a.B >= 0 && a.D > 0, "univariate backward: bad shape B=%lld D=%d", (long long)a.B, a.D);
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate backward: null input");
-    ZK_REQUIRE(a.univariate == ZK_UNI_AFFINE || a.univariate == ZK_UNI_RQS || a.univariate == ZK_UNI_GAUSS ||
-                   a.univariate == ZK_UNI_SOSP || a.univariate == ZK_UNI_BERNSTEIN,
-               "univariate backward: unknown kind %d", a.univariate);
-    if (a.univariate == ZK_UNI_RQS) {
-        ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "rqs backward: bins must be in [1, 1024], got %d", a.K);
-    } else if (a.univariate == ZK_UNI_GAUSS) {
-        ZK_REQUIRE(a.K >= 1 && a.K <= 1024, "gaussianization backward: components must be in [1, 1024], got %d", a.K);
-    } else if (a.univariate == ZK_UNI_SOSP) {
-        ZK_REQUIRE(sosp_shape_ok(a.K, a.degree), "sosp backward: polynomials %d / degree %d out of range", a.K, a.degree);
+    UniBwdPlan plan;
+    ZK_TRY(uni_bwd_plan(a.univariate, a.B, a.D, a.K, a.degree, a.phi_ld, plan));
+    if (a.univariate == ZK_UNI_SOSP) {
         ZK_REQUIRE(a.bound > 0.f, "sosp backward: bound must be positive");
     } else if (a.univariate == ZK_UNI_BERNSTEIN) {
-        ZK_REQUIRE(bernstein_shape_ok(a.degree), "bernstein backward: degree must be in [0, 59], got %d", a.degree);
         ZK_REQUIRE(a.bound > 0.f, "bernstein backward: bound must be positive");
         ZK_REQUIRE(a.eps > 0.f && a.eps < 0.5f, "bernstein backward: eps must be in (0, 1/2), got %g", (double)a.eps);
     }
-    const int P = uni_param_count(a.univariate, a.K, a.degree);
-    ZK_REQUIRE(a.phi_ld == 0 || a.phi_ld >= (int64_t)a.D * P, "univariate backward: phi_ld too small");
     ZK_REQUIRE(a.slope > 0.f && a.slope < 1.f, "univariate backward: slope must be in (0, 1)");
     ZK_REQUIRE(!(a.phi_ld == 0 && a.gphi == a.phi), "univariate backward: gphi cannot alias a shared table");
+    const int P = uni_param_count(a.univariate, a.K, a.degree);
     UniBwdParams p;
     p.x = a.x; p.ldx = a.ldx; p.phi = a.phi; p.phi_ld = a.phi_ld; p.gy = a.gy; p.ldgy = a.ldgy;
     p.gl = a.gl; p.gx = a.gx; p.ldgx = a.ldgx; p.gphi = a.gphi; p.dim_map = a.dim_map; p.B = a.B;
@@ -380,46 +418,36 @@ zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
     const float absL = fabsf(logf(a.slope));
     p.aw = 2.f / absL;
     p.ad = 1.f / absL;
-    const size_t row_bytes = (size_t)a.D * P * 4;
-    const size_t table = (a.phi_ld == 0) ? row_bytes : 0;
-    ZK_REQUIRE(row_bytes + table <= 200 * 1024, "univariate backward: D*P too large for one tile (%zu B)", row_bytes);
-    int64_t R = (int64_t)(24 * 1024 / row_bytes);
-    const int64_t r_pairs = ceil_div(kBwdThreads, a.D);
-    if (R < r_pairs) R = r_pairs;
-    while (R > 1 && R * row_bytes + table > 96 * 1024) --R;
-    if (R < 1) R = 1;
-    if (R > a.B) R = a.B;
-    p.rows_per_tile = (int)R;
-    const size_t smem = (size_t)R * row_bytes + table;
-    const int64_t grid = ceil_div(a.B, R);
-    ZK_REQUIRE(grid <= 0x7fffffff, "univariate backward: batch too large for one launch");
-    if (a.univariate == ZK_UNI_AFFINE) return launch_uni_bwd_t<ZK_UNI_AFFINE, 0>(p, a.fast_math, (int)grid, smem, stream);
+    p.rows_per_tile = plan.rows_per_tile;
+    const int grid = plan.grid;
+    const size_t smem = plan.smem;
+    const bool attr = plan.smem_attr;
+    if (a.univariate == ZK_UNI_AFFINE) return launch_uni_bwd_t<ZK_UNI_AFFINE, 0>(p, a.fast_math, grid, smem, attr, stream);
     if (a.univariate == ZK_UNI_GAUSS) {
-        switch (a.K) {
-            case 8: return launch_uni_bwd_t<ZK_UNI_GAUSS, 8>(p, a.fast_math, (int)grid, smem, stream);
-            case 16: return launch_uni_bwd_t<ZK_UNI_GAUSS, 16>(p, a.fast_math, (int)grid, smem, stream);
-            default: return launch_uni_bwd_t<ZK_UNI_GAUSS, 0>(p, a.fast_math, (int)grid, smem, stream);
+        switch (plan.kt) {
+            case 8: return launch_uni_bwd_t<ZK_UNI_GAUSS, 8>(p, a.fast_math, grid, smem, attr, stream);
+            case 16: return launch_uni_bwd_t<ZK_UNI_GAUSS, 16>(p, a.fast_math, grid, smem, attr, stream);
+            default: return launch_uni_bwd_t<ZK_UNI_GAUSS, 0>(p, a.fast_math, grid, smem, attr, stream);
         }
     }
     if (a.univariate == ZK_UNI_SOSP) {
         SospBwdParams sp;
         static_cast<UniBwdParams&>(sp) = p;
         sp.sosp = sosp::make_const(a.K, a.degree, a.bound, a.slope, 0);
-        if (a.K == sosp::kDefK && a.degree == sosp::kDefL)
-            return launch_uni_bwd_t<ZK_UNI_SOSP, sosp::kDefK>(sp, a.fast_math, (int)grid, smem, stream);
-        return launch_uni_bwd_t<ZK_UNI_SOSP, 0>(sp, a.fast_math, (int)grid, smem, stream);
+        if (plan.kt == sosp::kDefK) return launch_uni_bwd_t<ZK_UNI_SOSP, sosp::kDefK>(sp, a.fast_math, grid, smem, attr, stream);
+        return launch_uni_bwd_t<ZK_UNI_SOSP, 0>(sp, a.fast_math, grid, smem, attr, stream);
     }
     if (a.univariate == ZK_UNI_BERNSTEIN) {
         BernBwdParams bp;
         static_cast<UniBwdParams&>(bp) = p;
         bp.bern = bern::make_const(a.degree, a.bound, a.eps, 0);
-        if (P == bern::kDefP) return launch_uni_bwd_t<ZK_UNI_BERNSTEIN, bern::kDefP>(bp, a.fast_math, (int)grid, smem, stream);
-        return launch_uni_bwd_t<ZK_UNI_BERNSTEIN, 0>(bp, a.fast_math, (int)grid, smem, stream);
+        if (plan.kt == bern::kDefP) return launch_uni_bwd_t<ZK_UNI_BERNSTEIN, bern::kDefP>(bp, a.fast_math, grid, smem, attr, stream);
+        return launch_uni_bwd_t<ZK_UNI_BERNSTEIN, 0>(bp, a.fast_math, grid, smem, attr, stream);
     }
-    switch (a.K) {
-        case 8: return launch_uni_bwd_t<ZK_UNI_RQS, 8>(p, a.fast_math, (int)grid, smem, stream);
-        case 16: return launch_uni_bwd_t<ZK_UNI_RQS, 16>(p, a.fast_math, (int)grid, smem, stream);
-        default: return launch_uni_bwd_t<ZK_UNI_RQS, 0>(p, a.fast_math, (int)grid, smem, stream);
+    switch (plan.kt) {
+        case 8: return launch_uni_bwd_t<ZK_UNI_RQS, 8>(p, a.fast_math, grid, smem, attr, stream);
+        case 16: return launch_uni_bwd_t<ZK_UNI_RQS, 16>(p, a.fast_math, grid, smem, attr, stream);
+        default: return launch_uni_bwd_t<ZK_UNI_RQS, 0>(p, a.fast_math, grid, smem, attr, stream);
     }
 }
 

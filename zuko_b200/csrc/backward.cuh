@@ -17,7 +17,7 @@ namespace zk {
 
 // d(loss)/d(x, phi) of one univariate bijector pass.  gy (B, *) and gl (B) are the upstream
 // gradients of y and of the per-sample summed ladj (either may be null = 0).  gphi receives the
-// per-sample parameter gradients (B, D*P) (may alias phi when phi_ld == D*P); gx the direct
+// per-sample parameter gradients (B, D*P) (may be phi itself when phi_ld == D*P); gx the direct
 // input gradient (column dim_map[d] like the forward pass).
 struct UniBwdArgs {
     int univariate = ZK_UNI_RQS;
@@ -36,6 +36,19 @@ struct UniBwdArgs {
     bool circular = false;  // RQS: CircularShiftTransform(bound) in front (d shift / dx = 1)
     bool fast_math = false; // MUFU reciprocal / ex2 in the RQS and Gaussianization pair math (zk_set_fast_math)
 };
+
+// Tile plan of uni_bwd_kernel (launch_univariate_backward and zk_univariate_backward_plan both take it from
+// uni_bwd_plan).  A tile stages R parameter rows (or the shared table) and rewrites them with the gradients.
+struct UniBwdPlan {
+    int rows_per_tile = 0;        // R: ~24 KB of phi and >= ceil(256 / D) rows, shrunk to <= 96 KB with the table, capped by B
+    int grid = 0;                 // ceil(B / R) CTAs
+    size_t smem = 0;              // dynamic shared memory: R rows, plus the shared table unless it is rewritten in place
+    bool smem_attr = false;       // smem > 40 KB: the launch raises the dynamic shared memory attribute
+    bool table_in_place = false;  // shared table and R = 1: the kernel writes the gradients over the staged table
+    int kt = 0;                   // compile-time shape: RQS 8 / 16, Gaussianization 8 / 16, SOSP 3, Bernstein 17; 0 = runtime
+};
+// Validates the shape arguments as launch_univariate_backward does and fills `out`; B = 0 leaves it zero.  Host only.
+zk_status uni_bwd_plan(int uni, int64_t B, int D, int K, int degree, int64_t phi_ld, UniBwdPlan& out);
 zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream);
 
 // gx = gy / (1 + t)^2 - 2 gl sign(x) / (bound (1 + t)), t = |x| / bound  (transforms.py:309-316)
