@@ -491,6 +491,45 @@ zk_status zk_comm_group_begin(zk_comm* comm);
 zk_status zk_allreduce_sum(zk_comm* comm, int dev, double* buf, int n, zk_stream stream);
 zk_status zk_comm_group_end(zk_comm* comm);
 
+/* ------------------------------------------------------------------------- *
+ * Continuous normalizing flow: FreeFormJacobianTransform (zuko/transforms.py:1095-1179) with the vector field
+ * of FFJTransform.f (flows/continuous.py:88-97): f(t, x, c) = ode(cat(cos(freqs t), sin(freqs t), x, c)),
+ * integrated by adaptive Dormand-Prince (utils.py:443-554).  The step size is shared by the whole batch: the
+ * error of a trial is the maximum over every row and column, so a row's result depends on the rest of the
+ * batch through the step sequence, and one call integrates its whole batch (it never chunks it).
+ * Forward values only: no gradients through the integration.
+ * ------------------------------------------------------------------------- */
+#define ZK_CNF_TRACE_NONE 0       /* integrate x alone (_call / _inverse, transforms.py:1130-1144) */
+#define ZK_CNF_TRACE_EXACT 1      /* call_and_ladj with the exact trace of df/dx (transforms.py:1150-1174) */
+#define ZK_CNF_TRACE_HUTCHINSON 2 /* call_and_ladj with eps^T (df/dx) eps, eps supplied by the caller */
+
+typedef struct zk_cnf zk_cnf;
+
+/* ode: plain dense fp32 MLP (no masks, no residual blocks, any ZK_ACT_*) with dims[0] = features + context +
+ * 2 freqs and dims[n_linear] = features; freq_values: DEVICE float[freqs] (the module's `freqs` buffer).  The
+ * handle keeps a packed copy of the weights.  An MLP whose weights and per-row buffers do not fit one CTA's
+ * shared memory is refused with ZK_EUNSUPPORTED by zk_cnf_plan / zk_cnf_integrate. */
+zk_status zk_cnf_create(const zk_mlp_desc* ode, int features, int context, int freqs, const float* freq_values,
+                        zk_cnf** out);
+zk_status zk_cnf_destroy(zk_cnf* cnf);
+/* workspace of zk_cnf_integrate for B rows (a smaller one is ZK_EINVAL; it must be 256-byte aligned) */
+size_t zk_cnf_workspace_bytes(const zk_cnf* cnf, int64_t B, int trace);
+/* launch plan of zk_cnf_integrate: cooperative CTAs (co-resident CTAs per SM x SMs), threads per CTA (one row
+ * per thread and pass), passes over the rows per thread, dynamic shared memory; or the refusal status.  Outputs
+ * may be NULL.  No device work. */
+zk_status zk_cnf_plan(const zk_cnf* cnf, int64_t B, int trace, int* ctas, int* threads, int* passes, size_t* smem);
+/* Integrates x (B, D) with context c (B, C) (ldc = 0: one broadcast row; NULL when C = 0) from times[0] to
+ * times[1] (`times`: DEVICE float[2]; the inverse is the same call with the times swapped) with atol / rtol
+ * (utils.py:532-552).  trace: ZK_CNF_TRACE_*; eps (B, D), row stride ldeps, for ZK_CNF_TRACE_HUTCHINSON only.
+ * Writes y (B, D) (y may alias x) and, with a trace, ladj (B) = the integrated trace (NULL iff trace = NONE).
+ * counts: DEVICE int32[2] (trials, accepted steps) or NULL; step_log: DEVICE float[max_trials][4] (t, dt, error,
+ * accepted) per trial or NULL.  After max_trials trials without reaching times[1], or when t + dt == t in fp32
+ * (where the reference would loop forever), every output is NaN and counts[1] = -1 - accepted.  One cooperative launch, no host synchronisation. */
+zk_status zk_cnf_integrate(const zk_cnf* cnf, const float* x, int64_t ldx, const float* c, int64_t ldc, int64_t B,
+                           const float* times, float atol, float rtol, int trace, const float* eps, int64_t ldeps,
+                           int max_trials, float* y, int64_t ldy, float* ladj, int* counts, float* step_log,
+                           void* workspace, size_t ws_bytes, zk_stream stream);
+
 /* 1 (default): the conditioner GEMMs of the backward pass (forward recompute, dgrad, wgrad) of a
  * handle packed for the tensor cores run on them (split-bf16, fp32 accumulate); 0: fp32 FMA on
  * CUDA cores (exact-order arbitration path).  Returns the previous value. */

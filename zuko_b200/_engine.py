@@ -34,6 +34,7 @@ ZK_BASE_DIAG_NORMAL, ZK_BASE_BOX_UNIFORM = 0, 1
 ZK_GEMM_AUTO, ZK_GEMM_FP32, ZK_GEMM_BF16X3, ZK_GEMM_BF16X1 = range(4)
 (ZK_ACT_RELU, ZK_ACT_ELU, ZK_ACT_TANH, ZK_ACT_SILU, ZK_ACT_GELU, ZK_ACT_LEAKY_RELU, ZK_ACT_SOFTPLUS,
  ZK_ACT_SIGMOID) = (0, 2, 3, 4, 5, 6, 7, 8)  # fmt: skip
+ZK_CNF_TRACE_NONE, ZK_CNF_TRACE_EXACT, ZK_CNF_TRACE_HUTCHINSON = range(3)
 GEMM_MODES = {"auto": ZK_GEMM_AUTO, "fp32": ZK_GEMM_FP32, "bf16x3": ZK_GEMM_BF16X3, "bf16x1": ZK_GEMM_BF16X1}
 
 
@@ -178,6 +179,12 @@ _SIGNATURES = {
     "zk_flow_inverse_backward_min_workspace_bytes": (c_size_t, [POINTER(FlowDesc)]),
     "zk_flow_inverse_backward": (c_int, [POINTER(FlowDesc), _P, c_int64, _P, c_int64, c_int64, _P, c_int64, _P, _P, c_int64, _P, c_int64,
                                          _P, c_int64, POINTER(POINTER(LayerGrads)), _P, c_size_t, _P]),
+    "zk_cnf_create": (c_int, [POINTER(MlpDesc), c_int, c_int, c_int, _P, POINTER(c_void_p)]),
+    "zk_cnf_destroy": (c_int, [_P]),
+    "zk_cnf_workspace_bytes": (c_size_t, [_P, c_int64, c_int]),
+    "zk_cnf_plan": (c_int, [_P, c_int64, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_size_t)]),
+    "zk_cnf_integrate": (c_int, [_P, _P, c_int64, _P, c_int64, c_int64, _P, c_float, c_float, c_int, _P, c_int64, c_int, _P, c_int64,
+                                 _P, _P, _P, _P, c_size_t, _P]),
     "zk_flow_log_prob_host": (c_int, [POINTER(FlowDesc), _P, c_int64, _P, c_int64, c_int64, _P, POINTER(c_double), _P, c_size_t, _P]),
 }  # fmt: skip
 

@@ -29,6 +29,7 @@ import torch.nn as nn
 from . import distributions as _D
 from . import transforms as _T
 from .flows.autoregressive import MaskedAutoregressiveTransform
+from .flows.continuous import FFJTransform
 from .flows.coupling import GeneralCouplingTransform
 from .flows.elementwise import ElementWiseTransform
 from .lazy import (
@@ -157,6 +158,14 @@ def _convert(m: nn.Module, passthrough: bool = True) -> nn.Module:
                 univariate=_engine_callable(m.univariate), shapes=m.shapes, **kwargs,
             )  # fmt: skip
         return ElementWiseTransform(m.phi[0].shape[0], 0, univariate=_engine_callable(m.univariate), shapes=m.shapes)
+
+    if kind == "FFJTransform":  # zuko/flows/continuous.py:70-86
+        kwargs, linears = _conditioner_kwargs(m.ode)
+        kwargs.setdefault("activation", nn.ReLU)  # the reference's conditioner was built without an ELU default
+        F = m.freqs.numel()
+        D = linears[-1].weight.shape[0]
+        return FFJTransform(D, linears[0].weight.shape[1] - D - 2 * F, freqs=F, atol=m.atol, rtol=m.rtol, exact=m.exact,
+                            **kwargs)  # fmt: skip
 
     if kind in ("UnconditionalDistribution", "UnconditionalTransform"):  # zuko/lazy.py:242-335, utils.py:58-86
         if isinstance(m.f, nn.Module):

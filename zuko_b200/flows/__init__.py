@@ -1,6 +1,7 @@
 """Flow zoo of the hot path (zuko/flows/__init__.py, restricted to SURVEY §8)."""
 
 from .autoregressive import MAF, MaskedAutoregressiveTransform
+from .continuous import CNF, FFJTransform
 from .coupling import NICE, GeneralCouplingTransform, RealNVP
 from .elementwise import ElementWiseTransform
 from .gaussianization import GF
@@ -15,8 +16,10 @@ __all__ = [
     "NICE",
     "NSF",
     "BPF",
+    "CNF",
     "SOSPF",
     "ElementWiseTransform",
+    "FFJTransform",
     "Flow",
     "GeneralCouplingTransform",
     "MaskedAutoregressiveTransform",

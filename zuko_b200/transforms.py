@@ -14,6 +14,7 @@ C ABI of the H100 engine; no torch arithmetic runs here.
 * packed conditional layers produced by the lazy modules in ``zuko_b200.flows``:
   ``AutoregressiveTransform`` (:966-1007), ``CouplingTransform`` (:1010-1073),
   ``DependentTransform`` (:163-220, the element-wise case);
+* ``FreeFormJacobianTransform`` (:1095-1179), the continuous flow built by ``zuko_b200.flows.FFJTransform``;
 * ``ComposedTransform`` (:59-160), which hands a whole stack of packed layers to one
   flow-level engine call when it can.
 """
@@ -28,6 +29,7 @@ __all__ = [
     "ComposedTransform",
     "CouplingTransform",
     "DependentTransform",
+    "FreeFormJacobianTransform",
     "GaussianizationTransform",
     "MonotonicAffineTransform",
     "MonotonicRQSTransform",
@@ -893,3 +895,105 @@ class ComposedTransform(EngineTransform):
         for t in reversed(self.transforms):
             shape = t.inverse_shape(shape)
         return shape
+
+
+# --------------------------------------------------------------------------- #
+# continuous flow
+# --------------------------------------------------------------------------- #
+
+
+class FreeFormJacobianTransform(EngineTransform):
+    """Free-form Jacobian transformation ``x(t1) = x(t0) + int_t0^t1 f(t, x(t)) dt`` (transforms.py:1095-1179),
+    integrated by the engine's Dormand-Prince kernel (``zk_cnf_integrate``) with the step size shared by the
+    batch, as the reference does.  ``f`` is the vector field of :class:`zuko_b200.flows.FFJTransform` (built by
+    its ``forward``); an arbitrary Python callable is refused.  Leading dimensions are flattened into one batch,
+    which is integrated as a whole: the result of a row depends on the others through the step sequence.
+
+    ``exact=False`` estimates the trace with Hutchinson's ``eps^T (df/dx) eps``, ``eps = randn_like(x)`` drawn
+    once per call.  Forward values only: gradients through the integration (the reference's adaptive checkpoint
+    adjoint) are not implemented and are refused when they would be needed.  After ``max_trials`` trials without
+    reaching ``t1`` a call raises ``RuntimeError``."""
+
+    domain = constraints.real_vector
+    codomain = constraints.real_vector
+
+    def __init__(self, f, t0: float | Tensor = 0.0, t1: float | Tensor = 1.0, phi: Sequence[Tensor] = (),  # noqa: ANN001
+                 atol: float = 1e-6, rtol: float = 1e-5, exact: bool = True, max_trials: int = 10000) -> None:  # fmt: skip
+        super().__init__()
+        if not hasattr(f, "cnf_handle"):
+            raise NotImplementedError(
+                "zuko_b200: FreeFormJacobianTransform integrates the vector field of zuko_b200.flows.FFJTransform "
+                "only; an arbitrary Python callable is outside the engine"
+            )
+        self.f = f
+        self.t0, self.t1 = t0, t1
+        self.phi = tuple(p for p in phi if p.requires_grad)
+        self.atol, self.rtol, self.exact = atol, rtol, exact
+        self.max_trials = max_trials
+        self.stats = None  # (trials, accepted) of the last call
+
+    def __repr__(self) -> str:
+        return f"FreeFormJacobianTransform(exact={self.exact})"
+
+    @property
+    def inv(self) -> Transform:
+        return FreeFormJacobianTransform(self.f, self.t1, self.t0, self.phi, self.atol, self.rtol, self.exact, self.max_trials)
+
+    def _refuse_grad(self, x: Tensor) -> None:
+        # the rule of call_and_ladj's create_graph (transforms.py:1150): phi holds c and the ODE parameters in
+        # training mode only (flows/continuous.py:99-103)
+        if torch.is_grad_enabled() and (x.requires_grad or bool(self.phi)):
+            raise NotImplementedError(
+                "zuko_b200: gradients through the CNF integration (the adaptive checkpoint adjoint of "
+                "zuko/utils.py:556-593) are not implemented; call under torch.no_grad(), or use flow.eval() with "
+                "an input that does not require grad"
+            )
+
+    def _integrate(self, x: Tensor, trace: int) -> tuple[Tensor, Tensor | None]:
+        self._refuse_grad(x)
+        E.require_cuda(x, "CNF input")
+        D = x.shape[-1]
+        lead = x.shape[:-1]
+        x2 = x.reshape(-1, D)
+        if x2.stride(-1) != 1:
+            x2 = x2.contiguous()
+        B = x2.shape[0]
+        dev = x.device
+        times = torch.stack([torch.as_tensor(self.t0, device=dev), torch.as_tensor(self.t1, device=dev)]).float()
+        eps = torch.randn_like(x2) if trace == E.ZK_CNF_TRACE_HUTCHINSON else None
+        c, ldc = self.f.context(lead, B)
+        y = torch.empty(B, D, device=dev, dtype=torch.float32)
+        ladj = torch.empty(B, device=dev, dtype=torch.float32) if trace != E.ZK_CNF_TRACE_NONE else None
+        counts = torch.zeros(2, device=dev, dtype=torch.int32)
+        with torch.cuda.device(dev):
+            h = self.f.cnf_handle()
+            need = E.lib().zk_cnf_workspace_bytes(h, B, trace)
+            ws = E.Workspace.get(dev, need, need)
+            E.check(
+                E.lib().zk_cnf_integrate(
+                    h, x2.data_ptr(), x2.stride(0), c.data_ptr() if c is not None else None, ldc, B, times.data_ptr(),
+                    self.atol, self.rtol, trace, eps.data_ptr() if eps is not None else None, D, self.max_trials,
+                    y.data_ptr(), D, ladj.data_ptr() if ladj is not None else None, counts.data_ptr(), None,
+                    ws.data_ptr(), ws.numel(), E.stream_ptr(dev),
+                )
+            )  # fmt: skip
+        trials, accepted = counts.tolist()  # the one device-to-host read of a call
+        if accepted < 0:
+            raise RuntimeError(
+                f"zuko_b200: the CNF integration did not reach t1: {trials} trials (max_trials = {self.max_trials}), "
+                f"{-1 - accepted} accepted steps; the step size collapsed or the trial budget ran out"
+            )
+        self.stats = (trials, accepted)
+        return y.reshape(*lead, D), (ladj.reshape(lead) if ladj is not None else None)
+
+    def _call(self, x: Tensor) -> Tensor:
+        return self._integrate(x, E.ZK_CNF_TRACE_NONE)[0]
+
+    def _inverse(self, y: Tensor) -> Tensor:
+        return self.inv._call(y)
+
+    def call_and_ladj(self, x: Tensor) -> tuple[Tensor, Tensor]:
+        return self._integrate(x, E.ZK_CNF_TRACE_EXACT if self.exact else E.ZK_CNF_TRACE_HUTCHINSON)
+
+    def log_abs_det_jacobian(self, x: Tensor, y: Tensor) -> Tensor:
+        return self.call_and_ladj(x)[1]
