@@ -38,7 +38,7 @@ class _VectorField:
         E.require_cuda(c, "CNF context")
         if c.dim() == 1 or c.shape[:-1].numel() == 1:
             return c.reshape(1, -1).contiguous(), 0
-        c2 = c.expand(*lead, c.shape[-1]).reshape(B, -1)
+        c2 = c.expand(*lead, c.shape[-1]).reshape(B, c.shape[-1])  # -1 is ambiguous when B = 0
         if c2.stride(-1) != 1:
             c2 = c2.contiguous()
         return c2, c2.stride(0)

@@ -965,6 +965,9 @@ class FreeFormJacobianTransform(EngineTransform):
         y = torch.empty(B, D, device=dev, dtype=torch.float32)
         ladj = torch.empty(B, device=dev, dtype=torch.float32) if trace != E.ZK_CNF_TRACE_NONE else None
         counts = torch.zeros(2, device=dev, dtype=torch.int32)
+        if B == 0:  # nothing to integrate; the empty ladj and eps would reach the engine as NULL pointers
+            self.stats = (0, 0)
+            return y.reshape(*lead, D), (ladj.reshape(lead) if ladj is not None else None)
         with torch.cuda.device(dev):
             h = self.f.cnf_handle()
             need = E.lib().zk_cnf_workspace_bytes(h, B, trace)
