@@ -349,20 +349,35 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
         const int64_t row = rb + r;
         const bool row_ok = row < p.M;
         const float* bias = p.bias[L - 1];
-        // accumulators (+ bias) of output chunk ch -> this warpgroup's staging buffer
-        auto stage_chunk = [&](const float (&a)[NL / 2], int ch) {
+        // the bias pairs of output chunk ch that this thread adds to its accumulators
+        auto load_bias = [&](float2 (&bb)[NL / 8], int ch) {
+#pragma unroll
+            for (int i = 0; i < NL / 8; ++i) {
+                if (8 * i >= NP) break;
+                bb[i] = __ldg(reinterpret_cast<const float2*>(bias + ch * FK + 8 * i + 2 * (lane & 3)));
+            }
+        };
+        // accumulators + bias of output chunk ch -> this warpgroup's staging buffer
+        auto stage_chunk = [&](const float (&a)[NL / 2], const float2 (&bb)[NL / 8]) {
 #pragma unroll
             for (int i = 0; i < NL / 8; ++i) {
                 if (8 * i >= NP) break;
                 const int col = 8 * i + 2 * (lane & 3);
-                const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + ch * FK + col));
 #pragma unroll
                 for (int hh = 0; hh < 2; ++hh) {
                     float* dst = stg + (w * 16 + (lane >> 2) + 8 * hh) * SROW + col;
-                    if (col < NP) dst[0] = a[4 * i + 2 * hh] + bb.x;
-                    if (col + 1 < NP) dst[1] = a[4 * i + 2 * hh + 1] + bb.y;
+                    if (col < NP) dst[0] = a[4 * i + 2 * hh] + bb[i].x;
+                    if (col + 1 < NP) dst[1] = a[4 * i + 2 * hh + 1] + bb[i].y;
                 }
             }
+        };
+        // RQS: the input x of this thread's dim of output chunk ch (0 where the thread evaluates nothing)
+        auto load_x = [&](int ch) -> float {
+            if constexpr (UNI == ZK_UNI_RQS) {
+                const int d = ch * DPC + slot;
+                if (slot < DPC && d < p.D && row_ok) return __ldg(p.x + row * p.ldx + d);
+            }
+            return 0.f;
         };
         auto finish_dim = [&](float& ls, int d, float yv, float lj) {
             if (p.y) p.y[row * p.ldy + d] = yv;
@@ -374,8 +389,8 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
             }
             ls += lj;
         };
-        // bijector + log-derivative of this thread's dims of staged chunk ch, summed into ls
-        auto eval_chunk = [&](int ch, float& ls) {
+        // bijector + log-derivative of this thread's dims of staged chunk ch, summed into ls (RQS: xv = load_x(ch))
+        auto eval_chunk = [&](int ch, float& ls, float xv) {
             const float* pr = stg + r * SROW;
             if constexpr (UNI == ZK_UNI_RQS) {
                 if (slot < DPC) {
@@ -384,7 +399,6 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                         float pp[P];
 #pragma unroll
                         for (int j = 0; j < P; ++j) pp[j] = pr[slot * P + j];
-                        const float xv = __ldg(p.x + row * p.ldx + d);
                         float yv, lj;
                         Bin b = rqs_select<KT, FAST, false>(pp, KT, xv, p.bound, p.aw, p.ad);
                         rqs_forward_eval<FAST>(b, xv, yv, lj);
@@ -416,12 +430,17 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
             }
             // a chunk's tiles (at most F_WIDE_MAXKB <= n_stages) are multiplied as one batch of asynchronous MMAs and
             // released together once they are done.  The bijector runs with no MMAs in flight: its divergent
-            // branches inside a wgmma pipeline stage make ptxas serialize every wgmma of the kernel (C7515).
+            // branches inside a wgmma pipeline stage make ptxas serialize every wgmma of the kernel (C7515).  The
+            // chunk's bias and this thread's x are loaded before the batch is issued, so that their latency runs
+            // under the MMAs instead of after them.
             float acc[NL / 2];
             float ls0 = 0.f, ls1 = 0.f;  // partials of the even and of the odd chunks
             auto out_chunk = [&](int ch, float& ls) {
 #pragma unroll
                 for (int i = 0; i < NL / 2; ++i) acc[i] = 0.f;
+                float2 bb[NL / 8];
+                load_bias(bb, ch);
+                const float xv = load_x(ch);
                 const int hs = s;
                 int hn = 0;
                 for (int kb = 0; kb < nch; ++kb) {
@@ -437,9 +456,9 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                 wgmma_wait0();
                 acc_fence(acc);
                 for (int i = 0; i < hn; ++i) release((hs + i) % NS);
-                stage_chunk(acc, ch);
+                stage_chunk(acc, bb);
                 named_bar_sync(2 + cw, 128);
-                eval_chunk(ch, ls);
+                eval_chunk(ch, ls, xv);
                 named_bar_sync(2 + cw, 128);  // staging buffer free for the next chunk
             };
             for (int ch = 0; ch < p.n_last; ch += 2) {
@@ -465,9 +484,11 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                     }
                 }
                 if (!mine) continue;
-                stage_chunk(acc, ch);
+                float2 bb[NL / 8];
+                load_bias(bb, ch);
+                stage_chunk(acc, bb);
                 named_bar_sync(2 + cw, 128);
-                eval_chunk(ch, lsum);
+                eval_chunk(ch, lsum, load_x(ch));
                 named_bar_sync(2 + cw, 128);  // staging buffer free for the next chunk
             }
             part[(2 * cw + slot) * FM + r] = lsum;
