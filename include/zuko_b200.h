@@ -497,7 +497,7 @@ zk_status zk_comm_group_end(zk_comm* comm);
  * integrated by adaptive Dormand-Prince (utils.py:443-554).  The step size is shared by the whole batch: the
  * error of a trial is the maximum over every row and column, so a row's result depends on the rest of the
  * batch through the step sequence, and one call integrates its whole batch (it never chunks it).
- * Forward values only: no gradients through the integration.
+ * Gradients through the integration: zk_cnf_backward (the adaptive checkpoint adjoint, utils.py:556-593).
  * ------------------------------------------------------------------------- */
 #define ZK_CNF_TRACE_NONE 0       /* integrate x alone (_call / _inverse, transforms.py:1130-1144) */
 #define ZK_CNF_TRACE_EXACT 1      /* call_and_ladj with the exact trace of df/dx (transforms.py:1150-1174) */
@@ -529,6 +529,32 @@ zk_status zk_cnf_integrate(const zk_cnf* cnf, const float* x, int64_t ldx, const
                            const float* times, float atol, float rtol, int trace, const float* eps, int64_t ldeps,
                            int max_trials, float* y, int64_t ldy, float* ladj, int* counts, float* step_log,
                            void* workspace, size_t ws_bytes, zk_stream stream);
+
+/* Reverse mode of one zk_cnf_integrate call (AdaptiveCheckpointAdjoint.backward, utils.py:556-593, on the packed
+ * state (x, L) of call_and_ladj): for L = <grad_y, y> + <grad_ladj, ladj>.  x, c, ldc, B, trace and eps are the
+ * call's own; x is its INPUT.  step_log / trials / accepted are its device log and counts (trials, accepted).
+ * Each row is replayed from x along the logged accepted steps, bit for bit the call's states, then walked back
+ * one 6-stage Dormand-Prince step of -dt per step, second-order terms of the trace included.  The call's rows
+ * are independent once the steps are fixed, so the batch is processed in row chunks that fit the workspace.
+ * grad_y (may be NULL = 0); grad_ladj (B) non-NULL iff trace != NONE; eps non-NULL iff trace = HUTCHINSON.
+ * Writes grad_x (B, D) (may be NULL) and OVERWRITES grad_c ((B, C) rows, or one summed row when ldc == 0; may
+ * be NULL).  Weight and bias gradients are ACCUMULATED into grads (module (out, in) layout; NULL entries are not
+ * computed); reductions over rows run in a fixed order that does not depend on the chunking, so results are
+ * bit-identical run to run and for any workspace size.
+ * With no accepted step (t0 == t1) grad_x = grad_y and the rest is 0.  Ordinary launches, no host sync. */
+size_t zk_cnf_backward_workspace_bytes(const zk_cnf* cnf, int64_t B, int trace, int accepted); /* one chunk */
+/* chunks of one CTA's rows (threads per CTA) */
+size_t zk_cnf_backward_min_workspace_bytes(const zk_cnf* cnf, int trace, int accepted);
+/* threads per CTA (cnf_geometry's rule on the backward's per-row state), CTAs (co-resident x SMs), rows per chunk
+ * for this workspace, dynamic shared memory of the adjoint kernel; ZK_EUNSUPPORTED when the backward state does
+ * not fit; ZK_EINVAL when ws_bytes is below the minimum.  Outputs may be NULL.  No device work. */
+zk_status zk_cnf_backward_plan(const zk_cnf* cnf, int64_t B, int trace, int accepted, size_t ws_bytes, int* ctas,
+                               int* threads, int64_t* chunk_rows, size_t* smem);
+zk_status zk_cnf_backward(const zk_cnf* cnf, const float* x, int64_t ldx, const float* c, int64_t ldc, int64_t B,
+                          const float* step_log, int trials, int accepted, int trace, const float* eps, int64_t ldeps,
+                          const float* grad_y, int64_t ldgy, const float* grad_ladj, float* grad_x, int64_t ldgx,
+                          float* grad_c, int64_t ldgc, const zk_layer_grads* grads, void* workspace, size_t ws_bytes,
+                          zk_stream stream);
 
 /* 1 (default): the conditioner GEMMs of the backward pass (forward recompute, dgrad, wgrad) of a
  * handle packed for the tensor cores run on them (split-bf16, fp32 accumulate); 0: fp32 FMA on

@@ -185,6 +185,12 @@ _SIGNATURES = {
     "zk_cnf_plan": (c_int, [_P, c_int64, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_size_t)]),
     "zk_cnf_integrate": (c_int, [_P, _P, c_int64, _P, c_int64, c_int64, _P, c_float, c_float, c_int, _P, c_int64, c_int, _P, c_int64,
                                  _P, _P, _P, _P, c_size_t, _P]),
+    "zk_cnf_backward_workspace_bytes": (c_size_t, [_P, c_int64, c_int, c_int]),
+    "zk_cnf_backward_min_workspace_bytes": (c_size_t, [_P, c_int, c_int]),
+    "zk_cnf_backward_plan": (c_int, [_P, c_int64, c_int, c_int, c_size_t, POINTER(c_int), POINTER(c_int), POINTER(c_int64),
+                                     POINTER(c_size_t)]),
+    "zk_cnf_backward": (c_int, [_P, _P, c_int64, _P, c_int64, c_int64, _P, c_int, c_int, c_int, _P, c_int64, _P, c_int64, _P, _P,
+                                c_int64, _P, c_int64, POINTER(LayerGrads), _P, c_size_t, _P]),
     "zk_flow_log_prob_host": (c_int, [POINTER(FlowDesc), _P, c_int64, _P, c_int64, c_int64, _P, POINTER(c_double), _P, c_size_t, _P]),
 }  # fmt: skip
 

@@ -122,4 +122,18 @@ ZK_ACT_HD float act_deriv(float v, int act) {
     }
 }
 
+// d^2 act(v) / dv^2 at the PRE-activation v, with torch's double-backward conventions at the kinks (ELU's is 0
+// at v = 0, Softplus is linear above its threshold)
+ZK_ACT_HD float act_deriv2(float v, int act) {
+    switch (act) {
+        case ZK_ACT_ELU: return v >= 0.f ? 0.f : expf(v);
+        case ZK_ACT_TANH: { const float t = tanhf(v); return -2.f * t * (1.f - t * t); }
+        case ZK_ACT_SILU: { const float s = 1.f / (1.f + expf(-v)); return s * (1.f - s) * (2.f + v * (1.f - 2.f * s)); }
+        case ZK_ACT_GELU: return expf(-0.5f * v * v) * 0.39894228040143268f * (2.f - v * v);
+        case ZK_ACT_SOFTPLUS: { if (v > 20.f) return 0.f; const float s = 1.f / (1.f + expf(-v)); return s * (1.f - s); }
+        case ZK_ACT_SIGMOID: { const float s = 1.f / (1.f + expf(-v)); return s * (1.f - s) * (1.f - 2.f * s); }
+        default: return 0.f;  // ReLU, LeakyReLU, identity
+    }
+}
+
 }  // namespace zk

@@ -69,11 +69,11 @@ struct Params {
     int W, passes;
 };
 
-// out[o] = act(bias[o] + sum_j W[o, j] in(j)) (or, without bias, (sum_j W[o, j] in(j)) * scale[o]) for all
-// `pad` outputs, 8 at a time; per-thread buffers are strided by nt
-template <class In>
-__device__ __forceinline__ void dense(const float* __restrict__ WT, int pad, int n_in, const float* __restrict__ bias,
-                                      In in, float* out, int nt, int act, float* dact, const float* scale) {
+// bias[o] + sum_j W[o, j] in(j) (0 without bias) for all `pad` outputs, 8 at a time, each block of 8 handed to
+// epi(o0, acc)
+template <class In, class Epi>
+__device__ __forceinline__ void dense_to(const float* __restrict__ WT, int pad, int n_in, const float* __restrict__ bias,
+                                         In in, Epi epi) {
     for (int o0 = 0; o0 < pad; o0 += 8) {
         float acc[8];
 #pragma unroll
@@ -91,6 +91,16 @@ __device__ __forceinline__ void dense(const float* __restrict__ WT, int pad, int
             acc[6] = fmaf(w1.z, v, acc[6]);
             acc[7] = fmaf(w1.w, v, acc[7]);
         }
+        epi(o0, acc);
+    }
+}
+
+// out[o] = act(bias[o] + sum_j W[o, j] in(j)) (or, without bias, (sum_j W[o, j] in(j)) * scale[o]) for all
+// `pad` outputs, 8 at a time; per-thread buffers are strided by nt
+template <class In>
+__device__ __forceinline__ void dense(const float* __restrict__ WT, int pad, int n_in, const float* __restrict__ bias,
+                                      In in, float* out, int nt, int act, float* dact, const float* scale) {
+    dense_to(WT, pad, n_in, bias, in, [&](int o0, float (&acc)[8]) {
         if (dact) {
 #pragma unroll
             for (int r = 0; r < 8; ++r) dact[(o0 + r) * nt] = act_deriv(acc[r], act);
@@ -102,6 +112,31 @@ __device__ __forceinline__ void dense(const float* __restrict__ WT, int pad, int
         if (act) act_apply_n<8>(acc, act);
 #pragma unroll
         for (int r = 0; r < 8; ++r) out[(o0 + r) * nt] = acc[r];
+    });
+}
+
+// column j of stage s's state x + sum_m A[s][m] (dt f_m) of one row, f_m in slot(m) of Fk ((slots, W, B)
+// column-major); shared by the integration and the backward's replay, so the replayed states are bit for bit
+// the integration's
+template <class Slot>
+__device__ __forceinline__ float stage_state(const float* X, const float* Fk, int W, int64_t B, int64_t row, int j,
+                                             int s, float dt, Slot slot) {
+    float v = X[(int64_t)j * B + row];
+    for (int m = 0; m < s; ++m) {
+        const float k = __fmul_rn(dt, Fk[((int64_t)slot(m) * W + j) * B + row]);
+        if (kA[s][m] != 0.f) v = __fadd_rn(v, __fmul_rn(kA[s][m], k));
+    }
+    return v;
+}
+
+// time embedding (cos, sin)(freqs t_s) of the 7 stage times of a step (t, dt), by the CTA into emb (7, 2F)
+__device__ __forceinline__ void stage_embedding(const float* freqs, int F, float t, float dt, float* emb) {
+    for (int k = threadIdx.x; k < kStages * F; k += blockDim.x) {
+        const int s = k / F, i = k % F;
+        const float ts = __fadd_rn(t, __fmul_rn(kC[s], dt));
+        const float a = __fmul_rn(freqs[i], s >= 5 ? __fadd_rn(t, dt) : ts);
+        emb[s * 2 * F + i] = cosf(a);
+        emb[s * 2 * F + F + i] = sinf(a);
     }
 }
 
@@ -225,13 +260,7 @@ __global__ void __launch_bounds__(256, 1) cnf_dopri_kernel(Params p) {
             break;
         }
         __syncthreads();  // the previous trial's readers of emb are done
-        for (int k = tid; k < kStages * p.F; k += nt) {
-            const int s = k / p.F, i = k % p.F;
-            const float ts = __fadd_rn(t, __fmul_rn(kC[s], dt));
-            const float a = __fmul_rn(freqs[i], s >= 5 ? __fadd_rn(t, dt) : ts);
-            emb[s * F2 + i] = cosf(a);
-            emb[s * F2 + p.F + i] = sinf(a);
-        }
+        stage_embedding(freqs, p.F, t, dt, emb);
         __syncthreads();
 
         float emax = 0.f;
@@ -244,11 +273,7 @@ __global__ void __launch_bounds__(256, 1) cnf_dopri_kernel(Params p) {
             const float* cr = p.c ? p.c + row * p.ldc : nullptr;
             for (int s = have_f1 ? 1 : 0; s < kStages; ++s) {
                 for (int j = 0; j < D; ++j) {
-                    float v = Xc[(int64_t)j * B + row];
-                    for (int m = 0; m < s; ++m) {
-                        const float k = __fmul_rn(dt, p.Fk[((int64_t)slot(m) * W + j) * B + row]);
-                        if (kA[s][m] != 0.f) v = __fadd_rn(v, __fmul_rn(kA[s][m], k));
-                    }
+                    const float v = stage_state(Xc, p.Fk, W, B, row, j, s, dt, slot);
                     bufA[j * nt] = v;
                     if (s == kStages - 1) Xn[(int64_t)j * B + row] = v;
                 }
@@ -321,6 +346,354 @@ __global__ void __launch_bounds__(256, 1) cnf_dopri_kernel(Params p) {
         p.counts[0] = trials;
         p.counts[1] = failed ? -1 - accepted : accepted;
     }
+}
+
+// ---------------------------------------------------------------------------
+// Backward: AdaptiveCheckpointAdjoint.backward (utils.py:556-593) on the packed state (x, L) of call_and_ladj.
+// The accepted steps of the forward's log are known, so rows are independent: each row is replayed from x0
+// (cnf_replay_kernel, the integration's own stage arithmetic), then walked back one 6-stage Dormand-Prince step
+// of -dt per accepted step (cnf_adjoint_kernel) on (a, g_phi) with
+//   da/dt = -(a^T df/dx + a_L 1e-2 dtau/dx),   dg_phi/dt = -(a^T df/dphi + a_L 1e-2 dtau/dphi),
+// where tau = sum_k r_k^T (df/dx) s_k (exact: s_k = r_k = e_k, k < D; Hutchinson: s = r = eps) is differentiated
+// in reverse mode through the forward-mode tangent program, one tangent at a time, act'' included.  Since g_phi
+// never feeds the dynamics, g_phi += dt sum_s b_s VJP_phi(stage s): per stage, every thread adds the CTA's rows
+// (in order) of the outer products it owns into the CTA's partial; cnf_grad_reduce_kernel sums the partials in
+// CTA order.
+// ---------------------------------------------------------------------------
+constexpr int kAdjStages = 6;
+
+struct BackParams {
+    Params m;   // MLP shape and the chunk's x / c / eps (B = rows of the chunk); m.trace = NONE for the replay
+    int trace;  // the differentiated call's trace
+    int out[kMaxLinear], hoff[kMaxLinear];
+    int H, ns, passes;  // passes: the replay's
+    int64_t blk0;       // adjoint: global index of the chunk's first block of blockDim.x rows; block b of the whole
+    int gtot;           // call belongs to CTA b % gtot, whatever the chunking (bit-identical partials)
+    const float* log;
+    int trials, accepted;
+    const float* gy; int64_t ldgy;
+    const float* gl;
+    float* gx; int64_t ldgx;
+    float* gc; int64_t ldgc;  // per-row context gradient (ldc != 0) or NULL
+    float* Xs;    // (accepted + 1, D, R) replayed states
+    float* Fk;    // (7, D, R) stage values of f
+    float* Ka;    // (6, D, R) stage values of da/dt
+    float* Aa;    // (D, R) adjoint of x
+    float* Gc;    // (R, C) context gradient
+    float* part;  // (CTAs, wfloats) parameter-gradient partials in the packed weight layout
+};
+
+__global__ void __launch_bounds__(256) cnf_replay_kernel(BackParams q) {
+    extern __shared__ __align__(16) float smem[];
+    const Params& p = q.m;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    float* sw = smem;
+    float* emb = sw + p.wfloats;
+    float* bufA = emb + kStages * 2 * kMaxFreqs + tid;
+    float* bufB = bufA + (size_t)p.S * nt;
+    for (int k = tid; k < p.wfloats; k += nt) sw[k] = p.w[k];
+    const float* freqs = p.w + p.wfloats;
+    const int64_t R = p.B, stride = (int64_t)gridDim.x * nt, base = (int64_t)blockIdx.x * nt + tid;
+    const int D = p.D, F2 = 2 * p.F;
+    for (int ps = 0; ps < q.passes; ++ps) {
+        const int64_t row = base + ps * stride;
+        if (row >= R) break;
+        for (int j = 0; j < D; ++j) q.Xs[(int64_t)j * R + row] = p.x[row * p.ldx + j];
+    }
+    auto same = [](int m) { return m; };
+    int k = 0;
+    for (int i = 0; i < q.trials && k < q.accepted; ++i) {
+        if (q.log[4 * i + 3] == 0.f) continue;
+        const float t = q.log[4 * i], dt = q.log[4 * i + 1];
+        __syncthreads();
+        stage_embedding(freqs, p.F, t, dt, emb);
+        __syncthreads();
+        const float* Xc = q.Xs + (int64_t)k * D * R;
+        float* Xn = q.Xs + (int64_t)(k + 1) * D * R;
+        for (int ps = 0; ps < q.passes; ++ps) {
+            const int64_t row = base + ps * stride;
+            if (row >= R) break;
+            const float* cr = p.c ? p.c + row * p.ldc : nullptr;
+            for (int s = 0; s < kStages; ++s) {
+                for (int j = 0; j < D; ++j) {
+                    const float v = stage_state(Xc, q.Fk, D, R, row, j, s, dt, same);
+                    if (s == kStages - 1)
+                        Xn[(int64_t)j * R + row] = v;
+                    else
+                        bufA[j * nt] = v;
+                }
+                if (s == kStages - 1) break;
+                for (int j = 0; j < p.C; ++j) bufA[(D + j) * nt] = __ldg(cr + j);
+                eval_row(p, sw, emb + s * F2, bufA, bufB, nullptr, nt, row, q.Fk + (int64_t)s * D * R);
+            }
+        }
+        ++k;
+    }
+}
+
+// v_j = sum_{o < n_out} W[o, j] g[o] for j < n_in (g strided by ns), each handed to epi(j, v)
+template <class Epi>
+__device__ __forceinline__ void dense_t(const float* WT, int pad, int n_in, int n_out, const float* g, int ns, Epi epi) {
+    for (int j = 0; j < n_in; ++j) {
+        const float* w = WT + (size_t)j * pad;
+        float v = 0.f;
+        for (int o = 0; o < n_out; ++o) v = fmaf(w[o], g[o * ns], v);
+        epi(j, v);
+    }
+}
+
+// part[(j0 + j) pad + o] += wgt sum_r g[o][r] in(j, r) over the CTA's live rows r in order, for j < nj, o < n_out;
+// g is the CTA's buffer (row r at offset r, stride ns).  Each entry belongs to one thread: bit-reproducible.
+template <class In>
+__device__ __forceinline__ void reduce_outer(float* part, int pad, int j0, int nj, int n_out, const float* g, int ns,
+                                             const int* alive, float wgt, In in) {
+    const int nt = blockDim.x;
+    for (int e = threadIdx.x; e < nj * n_out; e += nt) {
+        const int j = e / n_out, o = e % n_out;
+        float s = 0.f;
+        for (int r = 0; r < nt; ++r)
+            if (alive[r]) s = fmaf(g[o * ns + r], in(j, r), s);
+        float* d = part + (size_t)(j0 + j) * pad + o;
+        *d = fmaf(wgt, s, *d);
+    }
+}
+
+__global__ void __launch_bounds__(256, 1) cnf_adjoint_kernel(BackParams q) {
+    extern __shared__ __align__(16) float smem[];
+    const Params& p = q.m;
+    const int tid = threadIdx.x, nt = blockDim.x, ns = q.ns;
+    const int D = p.D, C = p.C, F2 = 2 * p.F, nl = p.nl, L = nl - 1, H = q.H, S = p.S;
+    const bool tr = q.trace != ZK_CNF_TRACE_NONE, exact = q.trace == ZK_CNF_TRACE_EXACT;
+    float* sw = smem;
+    float* emb = sw + p.wfloats;
+    int* alive = reinterpret_cast<int*>(emb + kStages * 2 * kMaxFreqs);
+    // per-row buffers (row r at offset r, stride ns = nt + 1: the reductions read across rows without bank conflicts)
+    float* B_in = reinterpret_cast<float*>(alive + nt);  // x_s, c
+    float* B_h = B_in + (size_t)(D + C) * ns;            // act(pre) of the hidden layers
+    float* B_d = B_h + (size_t)H * ns;                   // act'(pre)
+    float* B_g0 = B_d + (size_t)H * ns;                  // three vectors of up to S
+    float* B_g1 = B_g0 + (size_t)S * ns;
+    float* B_g2 = B_g1 + (size_t)S * ns;
+    float* B_d2 = B_g2 + (size_t)S * ns;                 // with a trace: act''(pre)
+    float* B_u = B_d2 + (size_t)H * ns;                  // tangent of the hidden pre-activations
+    float* B_zb = B_u + (size_t)H * ns;                  // d tau / d pre of the hidden layers
+    float* B_e = B_zb + (size_t)H * ns;                  // Hutchinson eps
+    float *in = B_in + tid, *h = B_h + tid, *d = B_d + tid, *g0 = B_g0 + tid, *d2 = B_d2 + tid, *u = B_u + tid,
+          *zb = B_zb + tid, *e = B_e + tid;
+    for (int k = tid; k < p.wfloats; k += nt) sw[k] = p.w[k];
+    const float* freqs = p.w + p.wfloats;
+    float* part = q.part + (size_t)blockIdx.x * p.wfloats;
+    const int64_t R = p.B;
+    const float* W0 = sw + p.woff[0];
+    const int pad0 = p.pad[0];
+    auto same = [](int m) { return m; };
+
+    const int64_t nblk = (R + nt - 1) / nt;
+    const int64_t first = q.blk0 + ((blockIdx.x - q.blk0 % q.gtot) % q.gtot + q.gtot) % q.gtot;
+    for (int64_t blk = first; blk < q.blk0 + nblk; blk += q.gtot) {  // uniform over the CTA
+        const int64_t row = (blk - q.blk0) * nt + tid;
+        const bool live = row < R;
+        __syncthreads();
+        alive[tid] = live;
+        float alpha = 0.f;
+        const float* cr = nullptr;
+        if (live) {
+            for (int j = 0; j < D; ++j) q.Aa[(int64_t)j * R + row] = q.gy ? q.gy[row * q.ldgy + j] : 0.f;
+            for (int j = 0; j < C; ++j) q.Gc[row * C + j] = 0.f;
+            if (tr) alpha = __fmul_rn(__fmul_rn(q.gl[row], 100.f), kTraceScale);  // a_L = gl / 1e-2, times 1e-2
+            if (q.trace == ZK_CNF_TRACE_HUTCHINSON)
+                for (int j = 0; j < D; ++j) e[j * ns] = p.eps[row * p.ldeps + j];
+            cr = p.c ? p.c + row * p.ldc : nullptr;
+        }
+        int k = q.accepted;
+        for (int i = q.trials - 1; i >= 0 && k > 0; --i) {
+            if (q.log[4 * i + 3] == 0.f) continue;
+            const float dt = q.log[4 * i + 1];
+            const float tp = __fadd_rn(q.log[4 * i], dt), hs = -dt;  // from (t + dt, x_k) with step -dt
+            __syncthreads();
+            stage_embedding(freqs, p.F, tp, hs, emb);
+            __syncthreads();
+            const float* Xk = q.Xs + (int64_t)k * D * R;
+            for (int s = 0; s < kAdjStages; ++s) {
+                const float* es = emb + s * F2;
+                const float bs = kA[kStages - 1][s];
+                const bool wred = bs != 0.f;  // b_1 = 0: that stage feeds the later ones through a only
+                const float wgt = __fmul_rn(dt, bs);
+                if (live) {
+                    for (int j = 0; j < D; ++j) {
+                        in[j * ns] = stage_state(Xk, q.Fk, D, R, row, j, s, hs, same);
+                        g0[j * ns] = stage_state(q.Aa, q.Ka, D, R, row, j, s, hs, same);
+                    }
+                    for (int j = 0; j < C; ++j) in[(D + j) * ns] = __ldg(cr + j);
+                    // f at the stage, keeping act, act' (and act'') of every hidden layer
+                    for (int l = 0; l < nl; ++l) {
+                        const float* WT = sw + p.woff[l];
+                        const int ho = l < L ? q.hoff[l] : 0;
+                        auto epi = [&](int o0, float (&acc)[8]) {
+#pragma unroll
+                            for (int r = 0; r < 8; ++r) {
+                                const int o = o0 + r;
+                                if (l == L) {
+                                    if (o < D) q.Fk[((int64_t)s * D + o) * R + row] = acc[r];
+                                } else {
+                                    h[(ho + o) * ns] = act_apply(acc[r], p.act);
+                                    d[(ho + o) * ns] = act_deriv(acc[r], p.act);
+                                    if (tr) d2[(ho + o) * ns] = act_deriv2(acc[r], p.act);
+                                }
+                            }
+                        };
+                        if (l == 0)
+                            dense_to(WT, pad0, p.in[0], sw + p.boff[0], [&](int j) { return j < F2 ? es[j] : in[(j - F2) * ns]; }, epi);
+                        else {
+                            const int hi = q.hoff[l - 1];
+                            dense_to(WT, p.pad[l], p.in[l], sw + p.boff[l], [&](int j) { return h[(hi + j) * ns]; }, epi);
+                        }
+                    }
+                    if (tr)
+                        for (int o = 0; o < H; ++o) zb[o * ns] = 0.f;
+                }
+                // the trace term, one tangent at a time: forward tangent u, then back from a_L 1e-2 r
+                const int K = tr ? (exact ? D : 1) : 0;
+                for (int kk = 0; kk < K; ++kk) {
+                    float* ga = B_g1;
+                    float* gb = B_g2;
+                    if (live) {
+                        if (nl > 1) {
+                            if (exact)
+                                for (int o = 0; o < pad0; ++o) u[o * ns] = W0[(size_t)(F2 + kk) * pad0 + o];
+                            else
+                                dense_to(W0 + (size_t)F2 * pad0, pad0, D, nullptr, [&](int j) { return e[j * ns]; },
+                                         [&](int o0, float (&acc)[8]) {
+#pragma unroll
+                                             for (int r = 0; r < 8; ++r) u[(o0 + r) * ns] = acc[r];
+                                         });
+                            for (int l = 1; l < L; ++l) {
+                                const int hi = q.hoff[l - 1], ho = q.hoff[l];
+                                dense_to(sw + p.woff[l], p.pad[l], p.in[l], nullptr,
+                                         [&](int j) { return d[(hi + j) * ns] * u[(hi + j) * ns]; },
+                                         [&](int o0, float (&acc)[8]) {
+#pragma unroll
+                                             for (int r = 0; r < 8; ++r) u[(ho + o0 + r) * ns] = acc[r];
+                                         });
+                            }
+                        }
+                        for (int o = 0; o < D; ++o) ga[tid + o * ns] = exact ? (o == kk ? alpha : 0.f) : alpha * e[o * ns];
+                    }
+                    for (int l = L; l >= 1; --l) {
+                        const int hi = q.hoff[l - 1], nin = p.in[l], nout = q.out[l];
+                        if (wred) {
+                            __syncthreads();
+                            reduce_outer(part + p.woff[l], p.pad[l], 0, nin, nout, ga, ns, alive, wgt,
+                                         [&](int j, int r) { return B_d[(hi + j) * ns + r] * B_u[(hi + j) * ns + r]; });
+                            __syncthreads();
+                        }
+                        if (live) {
+                            float* gbo = gb + tid;
+                            dense_t(sw + p.woff[l], p.pad[l], nin, nout, ga + tid, ns, [&](int j, float v) {
+                                const int x2 = (hi + j) * ns;
+                                zb[x2] = fmaf(u[x2] * v, d2[x2], zb[x2]);
+                                gbo[j * ns] = d[x2] * v;
+                            });
+                        }
+                        float* t2 = ga;
+                        ga = gb;
+                        gb = t2;
+                    }
+                    if (wred) {
+                        __syncthreads();
+                        if (exact)
+                            reduce_outer(part + p.woff[0], pad0, F2 + kk, 1, q.out[0], ga, ns, alive, wgt,
+                                         [](int, int) { return 1.f; });
+                        else
+                            reduce_outer(part + p.woff[0], pad0, F2, D, q.out[0], ga, ns, alive, wgt,
+                                         [&](int j, int r) { return B_e[j * ns + r]; });
+                        __syncthreads();
+                    }
+                }
+                // reverse pass of f from a_s, the trace's d/d pre added at every hidden layer
+                float* ga = B_g0;
+                float* gb = B_g1;
+                for (int l = L; l >= 0; --l) {
+                    const int nin = p.in[l], nout = q.out[l];
+                    const int hi = l > 0 ? q.hoff[l - 1] : 0;
+                    if (wred) {
+                        __syncthreads();
+                        if (l == 0)
+                            reduce_outer(part + p.woff[0], pad0, 0, nin + 1, nout, ga, ns, alive, wgt, [&](int j, int r) {
+                                return j == nin ? 1.f : (j < F2 ? es[j] : B_in[(j - F2) * ns + r]);
+                            });
+                        else
+                            reduce_outer(part + p.woff[l], p.pad[l], 0, nin + 1, nout, ga, ns, alive, wgt,
+                                         [&](int j, int r) { return j == nin ? 1.f : B_h[(hi + j) * ns + r]; });
+                        __syncthreads();
+                    }
+                    if (live) {
+                        float* gbo = gb + tid;
+                        if (l > 0)
+                            dense_t(sw + p.woff[l], p.pad[l], nin, nout, ga + tid, ns, [&](int j, float v) {
+                                const int x2 = (hi + j) * ns;
+                                gbo[j * ns] = tr ? fmaf(d[x2], v, zb[x2]) : d[x2] * v;
+                            });
+                        else
+                            dense_t(W0 + (size_t)F2 * pad0, pad0, D + C, nout, ga + tid, ns, [&](int j, float v) {
+                                if (j < D) {
+                                    q.Ka[((int64_t)s * D + j) * R + row] = -v;
+                                } else if (wred) {
+                                    float* gcp = q.Gc + row * C + (j - D);
+                                    *gcp = fmaf(wgt, v, *gcp);
+                                }
+                            });
+                    }
+                    float* t2 = ga;
+                    ga = gb;
+                    gb = t2;
+                }
+            }
+            if (live)
+                for (int j = 0; j < D; ++j)
+                    q.Aa[(int64_t)j * R + row] = stage_state(q.Aa, q.Ka, D, R, row, j, kStages - 1, hs, same);
+            --k;
+        }
+        if (live) {
+            if (q.gx)
+                for (int j = 0; j < D; ++j) q.gx[row * q.ldgx + j] = q.Aa[(int64_t)j * R + row];
+            if (q.gc)
+                for (int j = 0; j < C; ++j) q.gc[row * q.ldgc + j] = q.Gc[row * C + j];
+        }
+    }
+}
+
+struct GradOut {
+    float* gw[kMaxLinear];
+    float* gb[kMaxLinear];
+    int in[kMaxLinear], out[kMaxLinear], pad[kMaxLinear], woff[kMaxLinear];
+    int nl, wfloats, ctas;
+    const float* part;
+};
+
+// one thread per packed entry: the CTA partials summed in CTA order, added into the (out, in) / (out) buffers
+__global__ void cnf_grad_reduce_kernel(GradOut g) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= g.wfloats) return;
+    int l = g.nl - 1;
+    while (l > 0 && e < g.woff[l]) --l;
+    const int rel = e - g.woff[l], j = rel / g.pad[l], o = rel % g.pad[l];
+    if (o >= g.out[l]) return;
+    float* dst = j < g.in[l] ? (g.gw[l] ? g.gw[l] + (size_t)o * g.in[l] + j : nullptr) : (g.gb[l] ? g.gb[l] + o : nullptr);
+    if (!dst) return;
+    float s = 0.f;
+    for (int c = 0; c < g.ctas; ++c) s += g.part[(size_t)c * g.wfloats + e];
+    *dst += s;
+}
+
+// grad_c (C) += the chunk's rows, one after the other in row order (a broadcast context): the same sequence of
+// additions whatever the chunking
+__global__ void cnf_context_sum_kernel(const float* Gc, int64_t R, int C, float* gc) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= C) return;
+    float s = gc[j];
+    for (int64_t r = 0; r < R; ++r) s += Gc[r * C + j];
+    gc[j] = s;
 }
 
 }  // namespace cnf
@@ -543,6 +916,232 @@ zk_status zk_cnf_integrate(const zk_cnf* h, const float* x, int64_t ldx, const f
     void* args[] = {&p};
     ZK_CUDA(cudaLaunchCooperativeKernel((const void*)cnf::cnf_dopri_kernel, dim3(g), dim3(nt), args, s, st));
     return check_launch("cnf_dopri_kernel");
+}
+
+}  // extern "C"
+
+namespace {
+
+// per-row floats of the adjoint kernel: x_s and c, act and act' of the hidden layers, three vectors of S, and
+// with a trace act'', the tangent, d tau / d pre and eps
+int cnf_back_thread_floats(const zk_cnf* h, int trace) {
+    return h->D + h->C + 2 * h->hidden_pad + 3 * h->S + (trace ? 3 * h->hidden_pad + h->D : 0);
+}
+
+size_t cnf_back_smem(const zk_cnf* h, int trace, int nt) {
+    return ((size_t)h->wfloats + cnf::kStages * 2 * cnf::kMaxFreqs + nt + (size_t)(nt + 1) * cnf_back_thread_floats(h, trace)) * 4;
+}
+
+size_t cnf_replay_smem(const zk_cnf* h, int nt) {
+    return ((size_t)h->wfloats + cnf::kStages * 2 * cnf::kMaxFreqs + (size_t)nt * 2 * h->S) * 4;
+}
+
+// threads per CTA by cnf_geometry's rule (the most resident threads per SM by shared memory, ties to more
+// threads), and co-resident CTAs of the adjoint kernel
+zk_status cnf_back_geometry(const zk_cnf* h, int trace, int* threads, size_t* smem, int* ctas) {
+    int best = 0;
+    size_t best_smem = 0;
+    int64_t best_res = 0;
+    for (int nt : cnf::kThreadChoices) {
+        const size_t s = cnf_back_smem(h, trace, nt);
+        if (s > cnf::kSmemCap) continue;
+        const int64_t per_sm = std::min<int64_t>({(int64_t)(cnf::kSmemPerSm / (s + 1024)), 2048 / nt, 32});
+        if (per_sm * nt > best_res) {
+            best_res = per_sm * nt;
+            best = nt;
+            best_smem = s;
+        }
+    }
+    if (!best)
+        return fail(ZK_EUNSUPPORTED, "cnf_backward: the MLP's backward state does not fit in shared memory (%zu bytes of "
+                    "weights, %d floats per row)", (size_t)h->wfloats * 4, cnf_back_thread_floats(h, trace));
+    ZK_CUDA(cudaFuncSetAttribute(cnf::cnf_adjoint_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)best_smem));
+    ZK_CUDA(cudaFuncSetAttribute(cnf::cnf_replay_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)cnf_replay_smem(h, best)));
+    int per_sm = 0;
+    ZK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cnf::cnf_adjoint_kernel, best, best_smem));
+    if (per_sm <= 0) return fail(ZK_EUNSUPPORTED, "cnf_backward: no CTA of %d threads and %zu bytes fits an SM", best, best_smem);
+    *threads = best;
+    *smem = best_smem;
+    *ctas = per_sm * sm_count();
+    return ZK_OK;
+}
+
+// workspace: the CTA partials, then per chunk row the replayed states, the stage values of f and da/dt, a and
+// the context gradient (five 256-byte aligned arrays)
+size_t cnf_back_fixed(const zk_cnf* h, int ctas) { return align_up((size_t)ctas * h->wfloats * 4, 256) + 5 * 256; }
+size_t cnf_back_row_bytes(const zk_cnf* h, int accepted) {
+    return ((size_t)(accepted + 1 + cnf::kStages + cnf::kAdjStages + 1) * h->D + h->C) * 4;
+}
+
+size_t cnf_back_ws(const zk_cnf* h, int64_t rows, int trace, int accepted) {
+    int nt = 0, g = 0;
+    size_t s = 0;
+    if (!h || rows < 0 || accepted < 0 || cnf_back_geometry(h, trace != ZK_CNF_TRACE_NONE, &nt, &s, &g) != ZK_OK) return 0;
+    return cnf_back_fixed(h, g) + (size_t)rows * cnf_back_row_bytes(h, accepted);
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t zk_cnf_backward_workspace_bytes(const zk_cnf* h, int64_t B, int trace, int accepted) {
+    return cnf_back_ws(h, B, trace, accepted);
+}
+
+size_t zk_cnf_backward_min_workspace_bytes(const zk_cnf* h, int trace, int accepted) {
+    int nt = 0, g = 0;
+    size_t s = 0;
+    if (!h || cnf_back_geometry(h, trace != ZK_CNF_TRACE_NONE, &nt, &s, &g) != ZK_OK) return 0;
+    return cnf_back_ws(h, nt, trace, accepted);
+}
+
+zk_status zk_cnf_backward_plan(const zk_cnf* h, int64_t B, int trace, int accepted, size_t ws_bytes, int* ctas,
+                               int* threads, int64_t* chunk_rows, size_t* smem) {
+    ZK_REQUIRE(h && B >= 0 && accepted >= 0, "cnf_backward_plan: bad argument");
+    ZK_REQUIRE(trace >= ZK_CNF_TRACE_NONE && trace <= ZK_CNF_TRACE_HUTCHINSON, "cnf_backward_plan: unknown trace %d", trace);
+    int nt = 0, g = 0;
+    size_t s = 0;
+    ZK_TRY(cnf_back_geometry(h, trace != ZK_CNF_TRACE_NONE, &nt, &s, &g));
+    const size_t fixed = cnf_back_fixed(h, g), row = cnf_back_row_bytes(h, accepted);
+    int64_t rows = 0;
+    if (B > 0) {  // whole blocks of nt rows per chunk, so that every row meets the same CTA whatever the chunking
+        const size_t least = fixed + (size_t)std::min<int64_t>(B, nt) * row;
+        ZK_REQUIRE(ws_bytes >= least, "cnf_backward_plan: workspace of %zu bytes given, %zu needed at least", ws_bytes, least);
+        const int64_t fit = (int64_t)((ws_bytes - fixed) / row);
+        rows = fit >= B ? B : fit / nt * nt;
+    }
+    if (ctas) *ctas = g;
+    if (threads) *threads = nt;
+    if (chunk_rows) *chunk_rows = rows;
+    if (smem) *smem = s;
+    return ZK_OK;
+}
+
+zk_status zk_cnf_backward(const zk_cnf* h, const float* x, int64_t ldx, const float* c, int64_t ldc, int64_t B,
+                          const float* step_log, int trials, int accepted, int trace, const float* eps, int64_t ldeps,
+                          const float* grad_y, int64_t ldgy, const float* grad_ladj, float* grad_x, int64_t ldgx,
+                          float* grad_c, int64_t ldgc, const zk_layer_grads* grads, void* workspace, size_t ws_bytes,
+                          zk_stream stream) {
+    ZK_REQUIRE(h, "cnf_backward: null handle");
+    ZK_REQUIRE(B >= 0, "cnf_backward: B=%lld", (long long)B);
+    ZK_REQUIRE(trace >= ZK_CNF_TRACE_NONE && trace <= ZK_CNF_TRACE_HUTCHINSON, "cnf_backward: unknown trace %d", trace);
+    ZK_REQUIRE(trials >= 0 && accepted >= 0 && accepted <= trials, "cnf_backward: trials=%d accepted=%d", trials, accepted);
+    ZK_REQUIRE(trials == 0 || step_log, "cnf_backward: null step_log");
+    ZK_REQUIRE((trace == ZK_CNF_TRACE_NONE) == (grad_ladj == nullptr),
+               "cnf_backward: grad_ladj must be NULL iff trace is NONE");
+    ZK_REQUIRE((trace == ZK_CNF_TRACE_HUTCHINSON) == (eps != nullptr) && (!eps || ldeps >= h->D),
+               "cnf_backward: eps (B, D) must be given iff trace is HUTCHINSON");
+    ZK_REQUIRE(!grad_y || ldgy >= h->D, "cnf_backward: ldgy=%lld", (long long)ldgy);
+    ZK_REQUIRE(!grad_x || ldgx >= h->D, "cnf_backward: ldgx=%lld", (long long)ldgx);
+    ZK_REQUIRE(h->C == 0 || (c && (ldc == 0 || ldc >= h->C)), "cnf_backward: bad context");
+    ZK_REQUIRE(!grad_c || h->C == 0 || ldc == 0 || ldgc >= h->C, "cnf_backward: ldgc=%lld", (long long)ldgc);
+    ZK_REQUIRE(B == 0 || (x && ldx >= h->D), "cnf_backward: bad x");
+    int nt = 0, g = 0;
+    size_t s = 0;
+    int64_t R = 0;
+    ZK_REQUIRE(((uintptr_t)workspace & 255) == 0, "cnf_backward: the workspace must be 256-byte aligned");
+    ZK_TRY(zk_cnf_backward_plan(h, B, trace, accepted, ws_bytes, &g, &nt, &R, &s));
+    ZK_REQUIRE(B == 0 || workspace, "cnf_backward: null workspace");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int C = h->C;
+    const bool csum = grad_c && C && ldc == 0;
+    if (csum) ZK_CUDA(cudaMemsetAsync(grad_c, 0, (size_t)C * 4, st));
+    if (B == 0) return ZK_OK;
+
+    char* ws = (char*)workspace;
+    float* part = (float*)ws;
+    ZK_CUDA(cudaMemsetAsync(part, 0, (size_t)g * h->wfloats * 4, st));
+    char* rows = ws + align_up((size_t)g * h->wfloats * 4, 256);
+    const int D = h->D;
+    float* Xs = (float*)rows;
+    float* Fk = (float*)((char*)Xs + align_up((size_t)(accepted + 1) * D * R * 4, 256));
+    float* Ka = (float*)((char*)Fk + align_up((size_t)cnf::kStages * D * R * 4, 256));
+    float* Aa = (float*)((char*)Ka + align_up((size_t)cnf::kAdjStages * D * R * 4, 256));
+    float* Gc = (float*)((char*)Aa + align_up((size_t)D * R * 4, 256));
+
+    cnf::BackParams q{};
+    cnf::Params& p = q.m;
+    p.w = h->w;
+    p.wfloats = h->wfloats;
+    p.nl = h->nl;
+    p.act = h->act;
+    p.D = D;
+    p.C = C;
+    p.F = h->F;
+    p.trace = ZK_CNF_TRACE_NONE;  // the replay integrates x alone
+    q.trace = trace;
+    int hoff = 0;
+    for (int l = 0; l < h->nl; ++l) {
+        p.in[l] = h->dims[l];
+        p.pad[l] = h->pad[l];
+        p.woff[l] = h->woff[l];
+        p.boff[l] = h->boff[l];
+        q.out[l] = h->dims[l + 1];
+        q.hoff[l] = hoff;
+        if (l < h->nl - 1) hoff += h->pad[l];
+    }
+    p.S = h->S;
+    p.W = D;
+    q.H = h->hidden_pad;
+    q.ns = nt + 1;
+    q.log = step_log;
+    q.trials = trials;
+    q.accepted = accepted;
+    q.Xs = Xs;
+    q.Fk = Fk;
+    q.Ka = Ka;
+    q.Aa = Aa;
+    q.Gc = Gc;
+    q.part = part;
+    const size_t replay_smem = cnf_replay_smem(h, nt);
+    q.gtot = (int)std::min<int64_t>(g, ceil_div(B, nt));
+    for (int64_t r0 = 0; r0 < B; r0 += R) {
+        const int64_t Rc = std::min<int64_t>(R, B - r0);
+        p.B = Rc;
+        p.x = x + r0 * ldx;
+        p.ldx = ldx;
+        p.c = C ? c + (ldc ? r0 * ldc : 0) : nullptr;
+        p.ldc = ldc;
+        p.eps = eps ? eps + r0 * ldeps : nullptr;
+        p.ldeps = ldeps;
+        q.gy = grad_y ? grad_y + r0 * ldgy : nullptr;
+        q.ldgy = ldgy;
+        q.gl = grad_ladj ? grad_ladj + r0 : nullptr;
+        q.gx = grad_x ? grad_x + r0 * ldgx : nullptr;
+        q.ldgx = ldgx;
+        q.gc = grad_c && C && ldc ? grad_c + r0 * ldgc : nullptr;
+        q.ldgc = ldgc;
+        const int grid = (int)std::min<int64_t>(g, ceil_div(Rc, nt));
+        q.passes = (int)ceil_div(Rc, (int64_t)grid * nt);
+        q.blk0 = r0 / nt;
+        cnf::cnf_replay_kernel<<<grid, nt, replay_smem, st>>>(q);
+        ZK_TRY(check_launch("cnf_replay_kernel"));
+        cnf::cnf_adjoint_kernel<<<q.gtot, nt, s, st>>>(q);
+        ZK_TRY(check_launch("cnf_adjoint_kernel"));
+        if (csum) {
+            cnf::cnf_context_sum_kernel<<<(C + 127) / 128, 128, 0, st>>>(Gc, Rc, C, grad_c);
+            ZK_TRY(check_launch("cnf_context_sum_kernel"));
+        }
+    }
+    if (grads && (grads->grad_weight || grads->grad_bias)) {
+        cnf::GradOut go{};
+        for (int l = 0; l < h->nl; ++l) {
+            go.gw[l] = grads->grad_weight ? grads->grad_weight[l] : nullptr;
+            go.gb[l] = grads->grad_bias ? grads->grad_bias[l] : nullptr;
+            go.in[l] = h->dims[l];
+            go.out[l] = h->dims[l + 1];
+            go.pad[l] = h->pad[l];
+            go.woff[l] = h->woff[l];
+        }
+        go.nl = h->nl;
+        go.wfloats = h->wfloats;
+        go.ctas = g;
+        go.part = part;
+        cnf::cnf_grad_reduce_kernel<<<(h->wfloats + 255) / 256, 256, 0, st>>>(go);
+        ZK_TRY(check_launch("cnf_grad_reduce_kernel"));
+    }
+    return ZK_OK;
 }
 
 }  // extern "C"

@@ -49,7 +49,8 @@ class FFJTransform(LazyTransform):
     ``ode(cat(cos(freqs t), sin(freqs t), x, c))`` of an :class:`zuko_b200.nn.MLP` (ELU by default) integrated
     from ``times[0]`` to ``times[1]``.  Same arguments, module tree (``ode``), buffers (``times``, ``freqs``),
     state-dict keys and seeded initialisation as the reference.  ``normalize=True`` and activations outside the
-    engine raise ``NotImplementedError``.  Forward values only: see :class:`FreeFormJacobianTransform`."""
+    engine raise ``NotImplementedError``.  ``adjoint=True`` (an engine extension, also settable afterwards) lets
+    the transforms it builds carry gradients through the integration: see :class:`FreeFormJacobianTransform`."""
 
     def __init__(
         self,
@@ -59,6 +60,7 @@ class FFJTransform(LazyTransform):
         atol: float = 1e-6,
         rtol: float = 1e-5,
         exact: bool = True,
+        adjoint: bool = False,
         **kwargs,
     ) -> None:
         super().__init__()
@@ -73,6 +75,7 @@ class FFJTransform(LazyTransform):
         self.atol = atol
         self.rtol = rtol
         self.exact = exact
+        self.adjoint = adjoint
 
     def _cnf_handle(self) -> ctypes.c_void_p:
         """The ``zk_cnf`` handle of the current weights, re-packed when a parameter or ``freqs`` changes."""
@@ -124,6 +127,7 @@ class FFJTransform(LazyTransform):
             atol=self.atol,
             rtol=self.rtol,
             exact=self.exact,
+            adjoint=self.adjoint,
         )
 
 

@@ -910,15 +910,19 @@ class FreeFormJacobianTransform(EngineTransform):
     which is integrated as a whole: the result of a row depends on the others through the step sequence.
 
     ``exact=False`` estimates the trace with Hutchinson's ``eps^T (df/dx) eps``, ``eps = randn_like(x)`` drawn
-    once per call.  Forward values only: gradients through the integration (the reference's adaptive checkpoint
-    adjoint) are not implemented and are refused when they would be needed.  After ``max_trials`` trials without
-    reaching ``t1`` a call raises ``RuntimeError``."""
+    once per call.  Gradients through the integration (the reference's adaptive checkpoint adjoint, second-order
+    terms of the trace included) are opt-in: with ``adjoint=True`` a call that can need them becomes one autograd
+    node whose backward is one ``zk_cnf_backward`` call; with ``adjoint=False`` (the default) such a call is
+    refused with ``NotImplementedError``.  Gradients reach ``x`` and the tensors of ``phi`` (the context and, in
+    training mode, the ODE parameters), never ``t0`` / ``t1``.  After ``max_trials`` trials without reaching
+    ``t1`` a call raises ``RuntimeError``."""
 
     domain = constraints.real_vector
     codomain = constraints.real_vector
 
     def __init__(self, f, t0: float | Tensor = 0.0, t1: float | Tensor = 1.0, phi: Sequence[Tensor] = (),  # noqa: ANN001
-                 atol: float = 1e-6, rtol: float = 1e-5, exact: bool = True, max_trials: int = 10000) -> None:  # fmt: skip
+                 atol: float = 1e-6, rtol: float = 1e-5, exact: bool = True, max_trials: int = 10000,
+                 adjoint: bool = False) -> None:  # fmt: skip
         super().__init__()
         if not hasattr(f, "cnf_handle"):
             raise NotImplementedError(
@@ -930,6 +934,7 @@ class FreeFormJacobianTransform(EngineTransform):
         self.phi = tuple(p for p in phi if p.requires_grad)
         self.atol, self.rtol, self.exact = atol, rtol, exact
         self.max_trials = max_trials
+        self.adjoint = adjoint
         self.stats = None  # (trials, accepted) of the last call
 
     def __repr__(self) -> str:
@@ -937,28 +942,28 @@ class FreeFormJacobianTransform(EngineTransform):
 
     @property
     def inv(self) -> Transform:
-        return FreeFormJacobianTransform(self.f, self.t1, self.t0, self.phi, self.atol, self.rtol, self.exact, self.max_trials)
+        return FreeFormJacobianTransform(self.f, self.t1, self.t0, self.phi, self.atol, self.rtol, self.exact, self.max_trials,
+                                         self.adjoint)  # fmt: skip
 
-    def _refuse_grad(self, x: Tensor) -> None:
+    def _needs_grad(self, x: Tensor) -> bool:
         # the rule of call_and_ladj's create_graph (transforms.py:1150): phi holds c and the ODE parameters in
         # training mode only (flows/continuous.py:99-103)
-        if torch.is_grad_enabled() and (x.requires_grad or bool(self.phi)):
+        if not (torch.is_grad_enabled() and (x.requires_grad or bool(self.phi))):
+            return False
+        if not self.adjoint:
             raise NotImplementedError(
                 "zuko_b200: gradients through the CNF integration (the adaptive checkpoint adjoint of "
-                "zuko/utils.py:556-593) are not implemented; call under torch.no_grad(), or use flow.eval() with "
-                "an input that does not require grad"
+                "zuko/utils.py:556-593) are opt-in: pass adjoint=True (or set transform.adjoint = True), call under "
+                "torch.no_grad(), or use flow.eval() with an input that does not require grad"
             )
+        if any(isinstance(t, Tensor) and t.requires_grad for t in (self.t0, self.t1)):
+            raise NotImplementedError("zuko_b200: gradients with respect to the CNF integration times are not implemented")
+        return True
 
-    def _integrate(self, x: Tensor, trace: int) -> tuple[Tensor, Tensor | None]:
-        self._refuse_grad(x)
-        E.require_cuda(x, "CNF input")
-        D = x.shape[-1]
-        lead = x.shape[:-1]
-        x2 = x.reshape(-1, D)
-        if x2.stride(-1) != 1:
-            x2 = x2.contiguous()
-        B = x2.shape[0]
-        dev = x.device
+    def _launch(self, x2: Tensor, lead: Size, trace: int, step_log: Tensor | None = None):
+        """One zk_cnf_integrate call on the rows x2 (B, D): (y, ladj or None, eps or None, c, ldc, trials, accepted)."""
+        B, D = x2.shape
+        dev = x2.device
         times = torch.stack([torch.as_tensor(self.t0, device=dev), torch.as_tensor(self.t1, device=dev)]).float()
         eps = torch.randn_like(x2) if trace == E.ZK_CNF_TRACE_HUTCHINSON else None
         c, ldc = self.f.context(lead, B)
@@ -967,7 +972,7 @@ class FreeFormJacobianTransform(EngineTransform):
         counts = torch.zeros(2, device=dev, dtype=torch.int32)
         if B == 0:  # nothing to integrate; the empty ladj and eps would reach the engine as NULL pointers
             self.stats = (0, 0)
-            return y.reshape(*lead, D), (ladj.reshape(lead) if ladj is not None else None)
+            return y, ladj, eps, c, ldc, 0, 0
         with torch.cuda.device(dev):
             h = self.f.cnf_handle()
             need = E.lib().zk_cnf_workspace_bytes(h, B, trace)
@@ -976,8 +981,8 @@ class FreeFormJacobianTransform(EngineTransform):
                 E.lib().zk_cnf_integrate(
                     h, x2.data_ptr(), x2.stride(0), c.data_ptr() if c is not None else None, ldc, B, times.data_ptr(),
                     self.atol, self.rtol, trace, eps.data_ptr() if eps is not None else None, D, self.max_trials,
-                    y.data_ptr(), D, ladj.data_ptr() if ladj is not None else None, counts.data_ptr(), None,
-                    ws.data_ptr(), ws.numel(), E.stream_ptr(dev),
+                    y.data_ptr(), D, ladj.data_ptr() if ladj is not None else None, counts.data_ptr(),
+                    step_log.data_ptr() if step_log is not None else None, ws.data_ptr(), ws.numel(), E.stream_ptr(dev),
                 )
             )  # fmt: skip
         trials, accepted = counts.tolist()  # the one device-to-host read of a call
@@ -987,6 +992,20 @@ class FreeFormJacobianTransform(EngineTransform):
                 f"{-1 - accepted} accepted steps; the step size collapsed or the trial budget ran out"
             )
         self.stats = (trials, accepted)
+        return y, ladj, eps, c, ldc, trials, accepted
+
+    def _integrate(self, x: Tensor, trace: int) -> tuple[Tensor, Tensor | None]:
+        grad = self._needs_grad(x)
+        E.require_cuda(x, "CNF input")
+        D = x.shape[-1]
+        lead = x.shape[:-1]
+        if grad:
+            out = _CNFAdjoint.apply(self, trace, x, *self.phi)
+            return (out, None) if trace == E.ZK_CNF_TRACE_NONE else out
+        x2 = x.reshape(-1, D)
+        if x2.stride(-1) != 1:
+            x2 = x2.contiguous()
+        y, ladj = self._launch(x2, lead, trace)[:2]
         return y.reshape(*lead, D), (ladj.reshape(lead) if ladj is not None else None)
 
     def _call(self, x: Tensor) -> Tensor:
@@ -1000,3 +1019,97 @@ class FreeFormJacobianTransform(EngineTransform):
 
     def log_abs_det_jacobian(self, x: Tensor, y: Tensor) -> Tensor:
         return self.call_and_ladj(x)[1]
+
+
+class _CNFAdjoint(torch.autograd.Function):
+    """One CNF integration as an autograd node with inputs ``(x, *phi)``: the forward logs its steps, the backward
+    is one ``zk_cnf_backward`` call (the adaptive checkpoint adjoint of zuko/utils.py:556-593).  The ODE
+    parameters are saved, so that modifying them in place between forward and backward raises as torch does, and
+    the handle looked up in backward is the forward's."""
+
+    @staticmethod
+    def forward(ctx, T: FreeFormJacobianTransform, trace: int, x: Tensor, *phi: Tensor):  # noqa: ANN001, ANN205
+        D = x.shape[-1]
+        lead = x.shape[:-1]
+        x2 = x.detach().reshape(-1, D)
+        if x2.stride(-1) != 1:
+            x2 = x2.contiguous()
+        B = x2.shape[0]
+        dev = x.device
+        owner = T.f.owner
+        with torch.cuda.device(dev):  # refuse a shape whose backward does not fit now, not at .backward()
+            E.check(E.lib().zk_cnf_backward_plan(T.f.cnf_handle(), 0, trace, 0, 0, None, None, None, None))
+        step_log = torch.empty(max(T.max_trials, 1), 4, device=dev, dtype=torch.float32)
+        y, ladj, eps, c, ldc, trials, accepted = T._launch(x2, lead, trace, step_log)
+        params = [t for m in owner.ode._linears() for t in (m.weight, m.bias) if t is not None]
+        ctx.save_for_backward(x2, c, eps, step_log, *params)
+        ctx.T, ctx.trace, ctx.lead, ctx.ldc = T, trace, lead, ldc
+        ctx.counts = (trials, accepted)
+        y = y.reshape(*lead, D)
+        if trace == E.ZK_CNF_TRACE_NONE:
+            return y
+        return y, ladj.reshape(lead)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gy: Tensor, gl: Tensor | None = None):  # noqa: ANN001, ANN205
+        x2, c, eps, step_log, *_ = ctx.saved_tensors
+        T, trace, lead, ldc = ctx.T, ctx.trace, ctx.lead, ctx.ldc
+        trials, accepted = ctx.counts
+        phi = T.phi
+        B, D = x2.shape
+        dev = x2.device
+        lins = T.f.owner.ode._linears()
+        gw = [torch.zeros_like(m.weight) if any(p is m.weight for p in phi) else None for m in lins]
+        gb = [torch.zeros_like(m.bias) if m.bias is not None and any(p is m.bias for p in phi) else None for m in lins]
+        cin = T.f.c
+        want_c = cin is not None and any(p is cin for p in phi)
+        gc = None
+        if want_c and c is not None:
+            gc = torch.empty(B, c.shape[-1], device=dev) if ldc else torch.empty(c.shape[-1], device=dev)
+        gx = torch.empty(B, D, device=dev) if ctx.needs_input_grad[2] else None
+        gy2 = None if gy is None else gy.reshape(B, D).float().contiguous()
+        gl2 = None
+        if trace != E.ZK_CNF_TRACE_NONE:
+            gl2 = torch.zeros(B, device=dev) if gl is None else gl.reshape(B).float().contiguous()
+        n = len(lins)
+        wp = (ctypes.c_void_p * n)(*[None if g is None else g.data_ptr() for g in gw])
+        bp = (ctypes.c_void_p * n)(*[None if g is None else g.data_ptr() for g in gb])
+        grads = E.LayerGrads()
+        grads.grad_weight, grads.grad_bias = wp, bp
+        if B:
+            with torch.cuda.device(dev):
+                h = T.f.cnf_handle()
+                lib = E.lib()
+                need = lib.zk_cnf_backward_workspace_bytes(h, B, trace, accepted)
+                ws = E.Workspace.get(dev, need, lib.zk_cnf_backward_min_workspace_bytes(h, trace, accepted))
+                E.check(
+                    lib.zk_cnf_backward(
+                        h, x2.data_ptr(), x2.stride(0), None if c is None else c.data_ptr(), ldc, B, step_log.data_ptr(),
+                        trials, accepted, trace, None if eps is None else eps.data_ptr(), D,
+                        None if gy2 is None else gy2.data_ptr(), D, None if gl2 is None else gl2.data_ptr(),
+                        None if gx is None else gx.data_ptr(), D, None if gc is None else gc.data_ptr(),
+                        c.shape[-1] if c is not None else 0, ctypes.byref(grads), ws.data_ptr(), ws.numel(),
+                        E.stream_ptr(dev),
+                    )
+                )  # fmt: skip
+        elif gx is not None:
+            gx.zero_()
+        out = []
+        for p in phi:
+            g = None
+            if p is cin:
+                if gc is None:
+                    g = torch.zeros_like(p)
+                elif ldc:
+                    g = gc.reshape(*lead, -1).sum_to_size(p.shape)
+                else:
+                    g = gc.reshape(p.shape)
+            else:
+                for m, w, b in zip(lins, gw, gb, strict=True):
+                    if p is m.weight:
+                        g = w
+                    elif p is m.bias:
+                        g = b
+            out.append(g)
+        return (None, None, None if gx is None else gx.reshape(*lead, D), *out)
