@@ -1093,8 +1093,10 @@ class _CNFAdjoint(torch.autograd.Function):
                         E.stream_ptr(dev),
                     )
                 )  # fmt: skip
-        elif gx is not None:
-            gx.zero_()
+        else:  # no rows: every gradient is zero, the broadcast context's included
+            for g in (gx, gc):
+                if g is not None:
+                    g.zero_()
         out = []
         for p in phi:
             g = None
@@ -1102,7 +1104,7 @@ class _CNFAdjoint(torch.autograd.Function):
                 if gc is None:
                     g = torch.zeros_like(p)
                 elif ldc:
-                    g = gc.reshape(*lead, -1).sum_to_size(p.shape)
+                    g = gc.reshape(*lead, gc.shape[-1]).sum_to_size(p.shape)  # -1 is ambiguous when B = 0
                 else:
                     g = gc.reshape(p.shape)
             else:
