@@ -73,7 +73,7 @@ zk_status zk_device_info(int* sm, int* major, int* minor) {
 zk_status zk_univariate_plan(int univariate, int64_t B, int D, int K, int degree, int64_t phi_ld, const float* phi,
                              int* rows_per_tile, size_t* smem, int* bulk_staging, int* shuffle_sum, int* bins_instantiated) {
     UniPlan p;
-    ZK_TRY(uni_plan(univariate, B, D, K, degree, phi_ld, phi, p));
+    ZK_TRY(uni_plan(UniSpec{univariate, K, degree}, B, D, phi_ld, phi, p));
     if (rows_per_tile) *rows_per_tile = p.rows_per_tile;
     if (smem) *smem = p.smem;
     if (bulk_staging) *bulk_staging = p.bulk ? 1 : 0;
@@ -82,84 +82,65 @@ zk_status zk_univariate_plan(int univariate, int64_t B, int D, int K, int degree
     return ZK_OK;
 }
 
+// one stand-alone pass: forward (x -> y, ladj) or inverse (x = the layer's output -> y = its input)
+static zk_status uni_entry(const UniSpec& spec, bool inverse, const float* x, int64_t ldx, const float* phi,
+                           int64_t phi_ld, int64_t B, int D, float* y, int64_t ldy, float* ladj, int accumulate,
+                           zk_stream stream) {
+    UniArgs a;
+    a.spec = spec; a.inverse = inverse; a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = phi_ld; a.B = B; a.D = D;
+    a.y = y; a.ldy = ldy; a.ladj = ladj; a.accumulate = accumulate;
+    a.fast_math = g_fast_math.load() != 0;
+    return launch_univariate(a, (cudaStream_t)stream);
+}
+
 zk_status zk_rqs_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
                          int D, int K, float bound, float slope, float* y, int64_t ldy, float* ladj,
                          int accumulate, zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_RQS; a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = phi_ld; a.B = B; a.D = D;
-    a.K = K; a.bound = bound; a.slope = slope; a.y = y; a.ldy = ldy; a.ladj = ladj;
-    a.accumulate = accumulate;
-    a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_RQS, K, 0, bound, slope}, false, x, ldx, phi, phi_ld, B, D, y, ldy, ladj, accumulate, stream);
 }
 
 zk_status zk_rqs_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B,
                          int D, int K, float bound, float slope, float* x, int64_t ldx,
                          zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_RQS; a.inverse = true; a.x = y; a.ldx = ldy; a.phi = phi; a.phi_ld = phi_ld;
-    a.B = B; a.D = D; a.K = K; a.bound = bound; a.slope = slope; a.y = x; a.ldy = ldx;
-    a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_RQS, K, 0, bound, slope}, true, y, ldy, phi, phi_ld, B, D, x, ldx, nullptr, 0, stream);
 }
 
 zk_status zk_affine_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
                             int D, float slope, float* y, int64_t ldy, float* ladj, int accumulate,
                             zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_AFFINE; a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = phi_ld; a.B = B;
-    a.D = D; a.slope = slope; a.y = y; a.ldy = ldy; a.ladj = ladj; a.accumulate = accumulate;
-    a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_AFFINE, 0, 0, 5.f, slope}, false, x, ldx, phi, phi_ld, B, D, y, ldy, ladj, accumulate, stream);
 }
 
 zk_status zk_affine_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B,
                             int D, float slope, float* x, int64_t ldx, zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_AFFINE; a.inverse = true; a.x = y; a.ldx = ldy; a.phi = phi;
-    a.phi_ld = phi_ld; a.B = B; a.D = D; a.slope = slope; a.y = x; a.ldy = ldx;
-    a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_AFFINE, 0, 0, 5.f, slope}, true, y, ldy, phi, phi_ld, B, D, x, ldx, nullptr, 0, stream);
 }
 
 zk_status zk_gaussianization_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
                                      int D, int K, float* y, int64_t ldy, float* ladj, int accumulate,
                                      zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_GAUSS; a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = phi_ld; a.B = B; a.D = D;
-    a.K = K; a.bound = 10.f; a.y = y; a.ldy = ldy; a.ladj = ladj; a.accumulate = accumulate;
-    a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_GAUSS, K, 0, 10.f}, false, x, ldx, phi, phi_ld, B, D, y, ldy, ladj, accumulate, stream);
 }
 
 zk_status zk_gaussianization_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B,
                                      int D, int K, float bound, int iterations, float* x, int64_t ldx,
                                      zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_GAUSS; a.inverse = true; a.x = y; a.ldx = ldy; a.phi = phi; a.phi_ld = phi_ld;
-    a.B = B; a.D = D; a.K = K; a.bound = bound; a.iters = iterations; a.y = x; a.ldy = ldx;
-    a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_GAUSS, K, 0, bound, 1e-3f, kBernsteinEps, iterations}, true, y, ldy, phi, phi_ld, B, D, x,
+                     ldx, nullptr, 0, stream);
 }
 
 zk_status zk_sosp_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
                           int K, int degree, float bound, float slope, float* y, int64_t ldy, float* ladj,
                           int accumulate, zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_SOSP; a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = phi_ld; a.B = B; a.D = D;
-    a.K = K; a.degree = degree; a.bound = bound; a.slope = slope; a.y = y; a.ldy = ldy; a.ladj = ladj;
-    a.accumulate = accumulate; a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_SOSP, K, degree, bound, slope}, false, x, ldx, phi, phi_ld, B, D, y, ldy, ladj, accumulate,
+                     stream);
 }
 
 zk_status zk_sosp_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B, int D,
                           int K, int degree, float bound, float slope, int iterations, float* x, int64_t ldx,
                           zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_SOSP; a.inverse = true; a.x = y; a.ldx = ldy; a.phi = phi; a.phi_ld = phi_ld;
-    a.B = B; a.D = D; a.K = K; a.degree = degree; a.bound = bound; a.slope = slope; a.iters = iterations;
-    a.y = x; a.ldy = ldx; a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_SOSP, K, degree, bound, slope, kBernsteinEps, iterations}, true, y, ldy, phi, phi_ld, B, D, x,
+                     ldx, nullptr, 0, stream);
 }
 
 // ceil(log2(2 bound / eps)) (MonotonicTransform._inverse, transforms.py:609-617); 0 when out of range
@@ -172,20 +153,14 @@ static int bisection_steps(float bound, float eps) {
 zk_status zk_bernstein_forward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
                                int degree, float bound, float eps, float* y, int64_t ldy, float* ladj,
                                int accumulate, zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_BERNSTEIN; a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = phi_ld; a.B = B; a.D = D;
-    a.degree = degree; a.bound = bound; a.eps = eps; a.y = y; a.ldy = ldy; a.ladj = ladj;
-    a.accumulate = accumulate; a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_BERNSTEIN, 0, degree, bound, 1e-3f, eps}, false, x, ldx, phi, phi_ld, B, D, y, ldy, ladj,
+                     accumulate, stream);
 }
 
 zk_status zk_bernstein_inverse(const float* y, int64_t ldy, const float* phi, int64_t phi_ld, int64_t B, int D,
                                int degree, float bound, float eps, float* x, int64_t ldx, zk_stream stream) {
-    UniArgs a;
-    a.univariate = ZK_UNI_BERNSTEIN; a.inverse = true; a.x = y; a.ldx = ldy; a.phi = phi; a.phi_ld = phi_ld;
-    a.B = B; a.D = D; a.degree = degree; a.bound = bound; a.eps = eps; a.iters = bisection_steps(bound, eps);
-    a.y = x; a.ldy = ldx; a.fast_math = g_fast_math.load() != 0;
-    return launch_univariate(a, (cudaStream_t)stream);
+    return uni_entry({ZK_UNI_BERNSTEIN, 0, degree, bound, 1e-3f, eps, bisection_steps(bound, eps)}, true, y, ldy, phi,
+                     phi_ld, B, D, x, ldx, nullptr, 0, stream);
 }
 
 zk_status zk_softclip_forward(const float* x, int64_t ldx, int64_t B, int D, float bound, float* y,
@@ -381,46 +356,25 @@ zk_status zk_layer_destroy(zk_layer* l) {
 }
 
 static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
-    l->kind = d->kind; l->D = d->features; l->C = d->context; l->uni = d->univariate;
-    if (l->uni == ZK_UNI_CRQS) {  // circular spline = shift + RQS over [-bound, bound] (flows/spline.py:65-72)
-        l->uni = ZK_UNI_RQS;
-        l->circ = true;
+    l->kind = d->kind; l->D = d->features; l->C = d->context; l->passes = d->passes;
+    l->spec = UniSpec{d->univariate, d->bins, d->degree, d->bound, d->slope, kBernsteinEps, d->iterations};
+    if (l->spec.kind == ZK_UNI_CRQS) {  // circular spline = shift + RQS over [-bound, bound] (flows/spline.py:65-72)
+        l->spec.kind = ZK_UNI_RQS;
+        l->spec.circular = true;
     }
-    l->K = d->bins; l->bound = d->bound; l->slope = d->slope; l->passes = d->passes; l->iters = d->iterations;
-    l->degree = d->degree;
     ZK_REQUIRE(l->D >= 1, "layer_create: features=%d", l->D);
     ZK_REQUIRE(l->C >= 0, "layer_create: context=%d", l->C);
     const bool has_uni = (l->kind == ZK_LAYER_AUTOREGRESSIVE || l->kind == ZK_LAYER_COUPLING ||
                           l->kind == ZK_LAYER_ELEMENTWISE);
     if (has_uni) {
-        ZK_REQUIRE(l->uni == ZK_UNI_AFFINE || l->uni == ZK_UNI_RQS || l->uni == ZK_UNI_GAUSS || l->uni == ZK_UNI_SOSP ||
-                       l->uni == ZK_UNI_BERNSTEIN,
-                   "layer_create: univariate=%d", d->univariate);
-        if (l->uni == ZK_UNI_GAUSS) {  // the bisection inverse is element-wise only (flows/gaussianization.py:97-155)
-            if (l->kind != ZK_LAYER_ELEMENTWISE)
-                return fail(ZK_EUNSUPPORTED, "layer_create: the Gaussianization bijector is supported in element-wise layers only");
-            ZK_REQUIRE(l->K >= 1 && l->K <= 1024, "layer_create: components=%d", l->K);
-            ZK_REQUIRE(l->bound > 0.f, "layer_create: bisection bound=%g", (double)l->bound);
-            ZK_REQUIRE(l->iters >= 1 && l->iters <= 64, "layer_create: bisection iterations=%d (must be in [1, 64])", l->iters);
-        }
-        if (l->uni == ZK_UNI_SOSP) {  // the bisection runs in autoregressive layers only (flows/polynomial.py:31-76)
-            if (l->kind != ZK_LAYER_AUTOREGRESSIVE)
-                return fail(ZK_EUNSUPPORTED, "layer_create: the SOSP bijector is supported in autoregressive layers only");
-            ZK_REQUIRE(sosp_shape_ok(l->K, l->degree),
-                       "layer_create: SOSP polynomials=%d degree=%d (degree <= 15, K (degree + 1) + 1 <= 1024)", l->K, l->degree);
-            ZK_REQUIRE(l->bound > 0.f, "layer_create: bisection bound=%g", (double)l->bound);
-            ZK_REQUIRE(l->iters >= 1 && l->iters <= 64, "layer_create: bisection iterations=%d (must be in [1, 64])", l->iters);
-        }
-        if (l->uni == ZK_UNI_BERNSTEIN) {  // BPF is a MAF (flows/polynomial.py:79-117): autoregressive layers only
-            if (l->kind != ZK_LAYER_AUTOREGRESSIVE)
-                return fail(ZK_EUNSUPPORTED, "layer_create: the Bernstein bijector is supported in autoregressive layers only");
-            ZK_REQUIRE(bernstein_shape_ok(l->degree), "layer_create: Bernstein degree=%d (must be in [0, 59])", l->degree);
-            ZK_REQUIRE(l->bound > 0.f, "layer_create: Bernstein bound=%g", (double)l->bound);
-            ZK_REQUIRE(l->iters >= 1 && l->iters <= 64, "layer_create: bisection iterations=%d (must be in [1, 64])", l->iters);
-        }
-        if (l->uni == ZK_UNI_RQS) ZK_REQUIRE(l->K >= 1 && l->K <= 1024, "layer_create: bins=%d", l->K);
-        ZK_REQUIRE(l->slope > 0.f && l->slope < 1.f, "layer_create: slope=%g", (double)l->slope);
-        l->P = uni_param_count(l->uni, l->K, l->degree);
+        const UniSpec& s = l->spec;
+        ZK_REQUIRE(uni_known(s.kind), "layer_create: univariate=%d", d->univariate);
+        if (!with_family(s.kind, [&](auto fam) { return (decltype(fam)::kLayers >> l->kind & 1) != 0; }))
+            return fail(ZK_EUNSUPPORTED, "layer_create: univariate=%d is not supported in layers of kind %d", d->univariate,
+                        l->kind);
+        ZK_TRY(uni_check_shape(s));
+        ZK_TRY(uni_check_scalars(s, true));
+        l->P = uni_P(s);
     }
     switch (l->kind) {
         case ZK_LAYER_AUTOREGRESSIVE: {
@@ -432,12 +386,12 @@ static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
             ZK_REQUIRE(l->hyper->dims[l->hyper->n_linear] == l->D * l->P,
                        "layer_create: conditioner out_features %d != D*P %d",
                        l->hyper->dims[l->hyper->n_linear], l->D * l->P);
-            ZK_TRY(fused_layer_prepare(l->hyper, d->hyper->mask, l->uni, l->K, l->D, l->C));
+            ZK_TRY(fused_layer_prepare(l->hyper, d->hyper->mask, l->spec.kind, l->spec.K, l->D, l->C));
             if (d->order) l->order.assign(d->order, d->order + l->D);
             {
                 int T = 0;
                 size_t smem = 0;
-                ZK_TRY(ar_inverse_pack(l->hyper, d->hyper->mask, d->order, l->D, l->C, l->uni, l->K, l->degree, l->passes, &l->inv));
+                ZK_TRY(ar_inverse_pack(l->hyper, d->hyper->mask, d->order, l->D, l->C, l->spec, l->passes, &l->inv));
                 if (l->inv && !ar_inverse_threads(l->inv, &T, &smem)) {  // state too large: use the sweeps
                     ar_inverse_free(l->inv);
                     l->inv = nullptr;
@@ -473,7 +427,7 @@ static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
             return ZK_OK;
         }
         case ZK_LAYER_SOFTCLIP:
-            ZK_REQUIRE(l->bound > 0.f, "layer_create: softclip bound=%g", (double)l->bound);
+            ZK_REQUIRE(l->spec.bound > 0.f, "layer_create: softclip bound=%g", (double)l->spec.bound);
             return ZK_OK;
         case ZK_LAYER_PERMUTATION: {
             ZK_REQUIRE(d->order, "layer_create: permutation needs order");
@@ -559,8 +513,8 @@ int zk_layer_fused_info(const zk_layer* l, double* out) {
     for (int i = 0; i < m->n_linear; ++i) dense += (double)m->dims[i] * m->dims[i + 1];
     out[3] = dense;
     const TcPack* pk = tc_pack_of(m);
-    if (!pk || l->circ || !fused_layer_supported(m, l->uni, l->K, l->D, l->C)) return 0;
-    const int kind = fused_layer_kind(m, l->uni, l->K, l->D, l->C);
+    if (!pk || l->spec.circular || !fused_layer_supported(m, l->spec.kind, l->spec.K, l->D, l->C)) return 0;
+    const int kind = fused_layer_kind(m, l->spec.kind, l->spec.K, l->D, l->C);
     out[0] = kind;
     out[1] = pk->fused.n_items;
     out[2] = pk->fused.issued_macs_per_row;
@@ -574,13 +528,13 @@ size_t zk_layer_fused_stream_bytes(const zk_layer* l) {
 }
 
 int zk_layer_fused_tile_rows(const zk_layer* l) {
-    if (!l || l->kind != ZK_LAYER_AUTOREGRESSIVE || !l->hyper || l->circ) return 0;
-    return fused_tile_rows(l->hyper, l->uni, l->K, l->D, l->C);
+    if (!l || l->kind != ZK_LAYER_AUTOREGRESSIVE || !l->hyper || l->spec.circular) return 0;
+    return fused_tile_rows(l->hyper, l->spec.kind, l->spec.K, l->D, l->C);
 }
 
 int zk_layer_fused_plan(const zk_layer* l, int* ring_slots, size_t* smem) {
-    if (!l || l->kind != ZK_LAYER_AUTOREGRESSIVE || !l->hyper || l->circ) return 0;
-    return fused_layer_plan(l->hyper, l->uni, l->K, l->D, l->C, ring_slots, smem);
+    if (!l || l->kind != ZK_LAYER_AUTOREGRESSIVE || !l->hyper || l->spec.circular) return 0;
+    return fused_layer_plan(l->hyper, l->spec.kind, l->spec.K, l->D, l->C, ring_slots, smem);
 }
 
 size_t zk_layer_workspace_bytes(const zk_layer* l, int64_t B) {
@@ -640,18 +594,18 @@ zk_status layer_forward_impl(const zk_layer* l, const float* x, int64_t ldx, con
     ZK_REQUIRE(l->C == 0 || c != nullptr, "layer needs a context of %d features", l->C);
     Arena ar(ws, ws_bytes);
     UniArgs a;
-    a.univariate = l->uni; a.B = B; a.K = l->K; a.degree = l->degree; a.bound = l->bound; a.slope = l->slope;
+    a.spec = l->spec; a.B = B;
     a.ladj = ladj; a.accumulate = accumulate; a.log_prob = log_prob; a.base_loc = loc;
-    a.base_scale = scale; a.fast_math = g_fast_math.load() != 0; a.circular = l->circ;
+    a.base_scale = scale; a.fast_math = g_fast_math.load() != 0;
     switch (l->kind) {
         case ZK_LAYER_AUTOREGRESSIVE: {
             // transforms.py:1005-1007 + flows/autoregressive.py:207-215
-            if (g_fused.load() && !l->circ && fused_layer_supported(l->hyper, l->uni, l->K, l->D, l->C)) {
+            if (g_fused.load() && !l->spec.circular && fused_layer_supported(l->hyper, l->spec.kind, l->spec.K, l->D, l->C)) {
                 // ONE kernel: conditioner GEMMs + bijector + ladj; neither the hidden
                 // activations nor phi touch HBM
                 FusedLayerArgs f;
-                f.univariate = l->uni; f.bins = l->K; f.D = l->D; f.C = l->C; f.bound = l->bound;
-                f.slope = l->slope; f.x = x; f.ldx = ldx; f.c = c; f.ldc = ldc; f.B = B; f.y = y; f.ldy = ldy;
+                f.univariate = l->spec.kind; f.bins = l->spec.K; f.D = l->D; f.C = l->C; f.bound = l->spec.bound;
+                f.slope = l->spec.slope; f.x = x; f.ldx = ldx; f.c = c; f.ldc = ldc; f.B = B; f.y = y; f.ldy = ldy;
                 f.ladj = ladj; f.accumulate = accumulate; f.log_prob = log_prob; f.base_loc = loc;
                 f.base_scale = scale; f.fast_math = g_fast_math.load() != 0;
                 return launch_fused_layer(l->hyper, f, st);
@@ -696,7 +650,7 @@ zk_status layer_forward_impl(const zk_layer* l, const float* x, int64_t ldx, con
             return launch_univariate(a, st);
         }
         case ZK_LAYER_SOFTCLIP:
-            return launch_softclip(x, ldx, B, l->D, l->bound, false, y, ldy, ladj, accumulate, st);
+            return launch_softclip(x, ldx, B, l->D, l->spec.bound, false, y, ldy, ladj, accumulate, st);
         case ZK_LAYER_PERMUTATION:
             ZK_TRY(launch_permute(x, ldx, l->perm, B, l->D, y, ldy, st));
             if (ladj && !accumulate) ZK_TRY(launch_fill(ladj, B, 0.f, st));  // transforms.py:1213-1214
@@ -722,8 +676,7 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
     ZK_REQUIRE(l->C == 0 || c != nullptr, "layer needs a context of %d features", l->C);
     Arena ar(ws, ws_bytes);
     UniArgs a;
-    a.univariate = l->uni; a.inverse = true; a.B = B; a.K = l->K; a.degree = l->degree; a.bound = l->bound; a.iters = l->iters;
-    a.slope = l->slope; a.fast_math = g_fast_math.load() != 0; a.circular = l->circ;
+    a.spec = l->spec; a.inverse = true; a.B = B; a.fast_math = g_fast_math.load() != 0;
     switch (l->kind) {
         case ZK_LAYER_AUTOREGRESSIVE: {
             // transforms.py:994-1000: x = zeros_like(y); for _ in range(passes): x = meta(x).inv(y)
@@ -738,7 +691,7 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
                     int T = 0;
                     size_t smem = 0;
                     ZK_TRY(ar_inverse_pack(ml->hyper, ml->hyper->mask.data(), ml->order.empty() ? nullptr : ml->order.data(), ml->D,
-                                           ml->C, ml->uni, ml->K, ml->degree, ml->passes, &ml->inv));
+                                           ml->C, ml->spec, ml->passes, &ml->inv));
                     if (ml->inv && !ar_inverse_threads(ml->inv, &T, &smem)) {
                         ar_inverse_free(ml->inv);
                         ml->inv = nullptr;
@@ -749,7 +702,7 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
             if (l->inv && g_fused.load()) {  // same fixed point, every weight visited once (ar_inverse.cu)
                 ArInvArgs ia;
                 ia.y = y; ia.ldy = ldy; ia.c = c; ia.ldc = ldc; ia.B = B; ia.x = x; ia.ldx = ldx;
-                ia.bound = l->bound; ia.slope = l->slope; ia.iters = l->iters; ia.fast = g_fast_math.load() != 0; ia.circular = l->circ;
+                ia.spec = l->spec; ia.fast = g_fast_math.load() != 0;
                 if (ladj) {
                     ia.ladj = ladj; ia.accumulate = accumulate; ia.base = base_lp; ia.base_loc = base_loc; ia.base_scale = base_scale;
                     ia.as_inverse_member = as_member;
@@ -804,7 +757,7 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
             return launch_univariate(a, st);
         }
         case ZK_LAYER_SOFTCLIP:
-            return launch_softclip(y, ldy, B, l->D, l->bound, true, x, ldx, nullptr, 0, st);
+            return launch_softclip(y, ldy, B, l->D, l->spec.bound, true, x, ldx, nullptr, 0, st);
         case ZK_LAYER_PERMUTATION:
             return launch_permute(y, ldy, l->perm_inv, B, l->D, x, ldx, st);
         case ZK_LAYER_ROTATION:
@@ -824,7 +777,7 @@ struct FlowPlan {
 // activations on chip: nothing), dir: 1 forward, 2 inverse, 0 either (the public, conservative figure)
 size_t layer_ws_dir(const zk_layer* l, int64_t Bc, int dir) {
     if (dir != 0 && l->kind == ZK_LAYER_AUTOREGRESSIVE && g_fused.load()) {
-        const bool fwd_fused = !l->circ && fused_layer_supported(l->hyper, l->uni, l->K, l->D, l->C);
+        const bool fwd_fused = !l->spec.circular && fused_layer_supported(l->hyper, l->spec.kind, l->spec.K, l->D, l->C);
         const bool inv_seq = (l->inv != nullptr || l->inv_dirty);
         if (dir == 1 && fwd_fused) return 0;
         if (dir == 2 && inv_seq) return 0;

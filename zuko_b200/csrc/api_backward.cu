@@ -310,7 +310,7 @@ zk_status layer_backward_impl(const zk_layer* l, const float* x, int64_t ldx, co
     ZK_REQUIRE(l->C == 0 || c != nullptr, "layer needs a context of %d features", l->C);
     Arena ar(ws, ws_bytes);
     UniBwdArgs u;
-    u.univariate = l->uni; u.B = B; u.K = l->K; u.degree = l->degree; u.bound = l->bound; u.slope = l->slope; u.circular = l->circ;
+    u.spec = l->spec; u.B = B;
     u.fast_math = g_fast_math.load() != 0;
     u.x = x; u.ldx = ldx; u.gy = gy; u.ldgy = ldgy; u.gl = gl; u.gx = gx; u.ldgx = ldgx;
     switch (l->kind) {
@@ -401,7 +401,7 @@ zk_status layer_backward_impl(const zk_layer* l, const float* x, int64_t ldx, co
             return ZK_OK;
         }
         case ZK_LAYER_SOFTCLIP:
-            return launch_softclip_backward(x, ldx, gy, ldgy, gl, B, l->D, l->bound, gx, ldgx, st);
+            return launch_softclip_backward(x, ldx, gy, ldgy, gl, B, l->D, l->spec.bound, gx, ldgx, st);
         case ZK_LAYER_PERMUTATION:  // y[:, j] = x[:, order[j]]  =>  gx[:, i] = gy[:, argsort(order)[i]]
             return launch_permute(gy, ldgy, l->perm_inv, B, l->D, gx, ldgx, st);
         case ZK_LAYER_ROTATION: {  // y = R x  =>  gx = R^T gy, gR += gy^T x
@@ -608,12 +608,14 @@ zk_status flow_inverse_backward_chunk(const zk_flow_desc* f, const float* x, int
     return ZK_OK;
 }
 
-zk_status uni_backward_entry(int uni, const float* x, int64_t ldx, const float* phi, int64_t phi_ld,
-                             int64_t B, int D, int K, float bound, float slope, const float* gy,
-                             int64_t ldgy, const float* gl, float* gx, int64_t ldgx, float* gphi,
-                             void* ws, size_t ws_bytes, cudaStream_t st, int degree = 0, float eps = kBernsteinEps) {
+zk_status uni_backward_entry(const UniSpec& spec, const float* x, int64_t ldx, const float* phi, int64_t phi_ld,
+                             int64_t B, int D, const float* gy, int64_t ldgy, const float* gl, float* gx, int64_t ldgx,
+                             float* gphi, void* ws, size_t ws_bytes, zk_stream stream, bool shape_first = false) {
+    const cudaStream_t st = (cudaStream_t)stream;
+    // the Gaussianization, SOSP and Bernstein entries refuse a bad shape even with B = 0; RQS and affine do not
+    if (shape_first) ZK_TRY(uni_check_shape(spec));
     ZK_REQUIRE(x && phi && B >= 0 && D > 0, "univariate backward: bad arguments");
-    const int P = uni_param_count(uni, K, degree);
+    const int P = uni_P(spec);
     if (gphi != nullptr && B > 0 && P > 0) {
         // grad_phi may only be phi itself with dense rows: each tile then rewrites the rows it staged.  Any
         // other overlap lets one CTA's (or one chunk's) writes reach parameters another one still reads
@@ -625,7 +627,7 @@ zk_status uni_backward_entry(int uni, const float* x, int64_t ldx, const float* 
                    "univariate backward: grad_phi overlaps phi (only grad_phi == phi with phi_ld == D*P is allowed)");
     }
     UniBwdArgs u;
-    u.univariate = uni; u.K = K; u.degree = degree; u.bound = bound; u.slope = slope; u.eps = eps; u.D = D;
+    u.spec = spec; u.D = D;
     u.fast_math = g_fast_math.load() != 0;
     u.phi = phi; u.phi_ld = phi_ld;
     if (phi_ld != 0 || gphi == nullptr) {
@@ -658,7 +660,7 @@ int zk_set_tc_backward(int on) { return g_tc_backward.exchange(on ? 1 : 0); }
 zk_status zk_univariate_backward_plan(int univariate, int64_t B, int D, int K, int degree, int64_t phi_ld,
                                       int* rows_per_tile, size_t* smem, int* instantiated) {
     UniBwdPlan p;
-    ZK_TRY(uni_bwd_plan(univariate, B, D, K, degree, phi_ld, p));
+    ZK_TRY(uni_bwd_plan(UniSpec{univariate, K, degree}, B, D, phi_ld, p));
     if (rows_per_tile) *rows_per_tile = p.rows_per_tile;
     if (smem) *smem = p.smem;
     if (instantiated) *instantiated = p.kt;
@@ -674,43 +676,40 @@ zk_status zk_rqs_backward(const float* x, int64_t ldx, const float* phi, int64_t
                           int D, int K, float bound, float slope, const float* grad_y, int64_t ldgy,
                           const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi,
                           void* ws, size_t ws_bytes, zk_stream stream) {
-    return uni_backward_entry(ZK_UNI_RQS, x, ldx, phi, phi_ld, B, D, K, bound, slope, grad_y, ldgy, grad_ladj,
-                              grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream);
+    return uni_backward_entry({ZK_UNI_RQS, K, 0, bound, slope}, x, ldx, phi, phi_ld, B, D, grad_y, ldgy, grad_ladj,
+                              grad_x, ldgx, grad_phi, ws, ws_bytes, stream);
 }
 
 zk_status zk_affine_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
                              int D, float slope, const float* grad_y, int64_t ldgy,
                              const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi,
                              void* ws, size_t ws_bytes, zk_stream stream) {
-    return uni_backward_entry(ZK_UNI_AFFINE, x, ldx, phi, phi_ld, B, D, 0, 5.f, slope, grad_y, ldgy, grad_ladj,
-                              grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream);
+    return uni_backward_entry({ZK_UNI_AFFINE, 0, 0, 5.f, slope}, x, ldx, phi, phi_ld, B, D, grad_y, ldgy, grad_ladj,
+                              grad_x, ldgx, grad_phi, ws, ws_bytes, stream);
 }
 
 zk_status zk_gaussianization_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B,
                                       int D, int K, const float* grad_y, int64_t ldgy, const float* grad_ladj,
                                       float* grad_x, int64_t ldgx, float* grad_phi, void* ws, size_t ws_bytes,
                                       zk_stream stream) {
-    ZK_REQUIRE(K >= 1 && K <= 1024, "gaussianization backward: components must be in [1, 1024], got %d", K);
-    return uni_backward_entry(ZK_UNI_GAUSS, x, ldx, phi, phi_ld, B, D, K, 10.f, 1e-3f, grad_y, ldgy, grad_ladj,
-                              grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream);
+    return uni_backward_entry({ZK_UNI_GAUSS, K, 0, 10.f}, x, ldx, phi, phi_ld, B, D, grad_y, ldgy, grad_ladj, grad_x, ldgx,
+                              grad_phi, ws, ws_bytes, stream, true);
 }
 
 zk_status zk_sosp_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
                            int K, int degree, float bound, float slope, const float* grad_y, int64_t ldgy,
                            const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi, void* ws,
                            size_t ws_bytes, zk_stream stream) {
-    ZK_REQUIRE(sosp_shape_ok(K, degree), "sosp backward: polynomials %d / degree %d out of range", K, degree);
-    return uni_backward_entry(ZK_UNI_SOSP, x, ldx, phi, phi_ld, B, D, K, bound, slope, grad_y, ldgy, grad_ladj,
-                              grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream, degree);
+    return uni_backward_entry({ZK_UNI_SOSP, K, degree, bound, slope}, x, ldx, phi, phi_ld, B, D, grad_y, ldgy,
+                              grad_ladj, grad_x, ldgx, grad_phi, ws, ws_bytes, stream, true);
 }
 
 zk_status zk_bernstein_backward(const float* x, int64_t ldx, const float* phi, int64_t phi_ld, int64_t B, int D,
                                 int degree, float bound, float eps, const float* grad_y, int64_t ldgy,
                                 const float* grad_ladj, float* grad_x, int64_t ldgx, float* grad_phi, void* ws,
                                 size_t ws_bytes, zk_stream stream) {
-    ZK_REQUIRE(bernstein_shape_ok(degree), "bernstein backward: degree must be in [0, 59], got %d", degree);
-    return uni_backward_entry(ZK_UNI_BERNSTEIN, x, ldx, phi, phi_ld, B, D, 0, bound, 1e-3f, grad_y, ldgy, grad_ladj,
-                              grad_x, ldgx, grad_phi, ws, ws_bytes, (cudaStream_t)stream, degree, eps);
+    return uni_backward_entry({ZK_UNI_BERNSTEIN, 0, degree, bound, 1e-3f, eps}, x, ldx, phi, phi_ld, B, D, grad_y, ldgy,
+                              grad_ladj, grad_x, ldgx, grad_phi, ws, ws_bytes, stream, true);
 }
 
 zk_status zk_softclip_backward(const float* x, int64_t ldx, int64_t B, int D, float bound,

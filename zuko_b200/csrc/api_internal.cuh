@@ -9,6 +9,7 @@
 #include "fused_layer.cuh"
 #include "mlp.cuh"
 #include "mlp_tcgen05.cuh"
+#include "uni_family.cuh"
 
 namespace zk {
 
@@ -48,11 +49,8 @@ inline zk_status dev_copy_from_host(const T* host, size_t n, T** out) {
 // layer handle
 // ===========================================================================
 struct zk_layer {
-    int kind = 0, D = 0, C = 0, uni = 0, K = 0, P = 0, passes = 0;
-    int iters = 0;                 // ZK_UNI_GAUSS / ZK_UNI_SOSP: bisection steps of the inverse
-    int degree = 0;                // ZK_UNI_SOSP: polynomial degree (K = polynomials)
-    float bound = 5.f, slope = 1e-3f;
-    bool circ = false;             // ZK_UNI_CRQS: CircularShiftTransform(bound) in front of the spline
+    int kind = 0, D = 0, C = 0, P = 0, passes = 0;
+    zk::UniSpec spec;              // the bijector (ZK_UNI_CRQS: RQS + circular); spec.bound is also the softclip bound
     zk_mlp* hyper = nullptr;       // owned
     float* phi_shared = nullptr;   // device (D, P), owned
     float* rotation = nullptr;     // device (D, D), owned

@@ -10,9 +10,8 @@
 //   step p = 0 .. passes-1:
 //     every hidden unit whose inputs became final at step p is computed;
 //     the P parameter rows of every dim of class p are computed from the last hidden layer;
-//     the inverse bijector (transforms.py:534-548 / 443-444, or the SOSP / Bernstein bisection of
-//     transforms.py:609-617, 807-831 in registers) yields x_d, which is stored and becomes an input of
-//     the later steps.
+//     the family's inverse (uni_family.cuh: inverse_ladj, in registers) yields x_d, which is stored and
+//     becomes an input of the later steps.
 //
 // This visits every weight once instead of `passes` times and reproduces the reference's fixed
 // point up to summation order (SURVEY §3.2, §7.2).  The same sweep also yields what
@@ -42,12 +41,12 @@
 
 #include "activations.cuh"
 #include "ar_inverse.cuh"
-#include "bijector_math.cuh"
+#include "uni_family.cuh"
 
 namespace zk {
 
 struct ArInvPack {
-    int D = 0, C = 0, P = 0, uni = 0, bins = 0, degree = 0, passes = 0, act = 1;
+    int D = 0, C = 0, P = 0, uni = 0, kt = 0, passes = 0, act = 1;
     int n_linear = 0;
     std::vector<int> dims;         // n_linear + 1
     std::vector<int> sec_off;      // state section offsets (floats): IN, H1 .. H_{L-1}, end
@@ -127,8 +126,7 @@ __device__ __forceinline__ void tile_dot(const float* __restrict__ w, const floa
 //           then per dim ONE block of its PT tiles: K x (PT * 8) weights k-major + PT * 8 biases
 template <int UNI, int KT, bool FAST, int R, bool GACT>
 __global__ void __launch_bounds__(256) ar_inverse_kernel(const InvParams p) {
-    constexpr int P = (UNI == ZK_UNI_RQS) ? 3 * KT - 1
-                    : (UNI == ZK_UNI_SOSP ? sosp::kDefP : (UNI == ZK_UNI_BERNSTEIN ? bern::kDefP : 2));
+    constexpr int P = UniFamily<UNI>::fixed_P(KT);
     constexpr int PT = (P + TILE - 1) / TILE;  // tiles per dim
     extern __shared__ __align__(16) float state[];  // [state_floats][S], S = R * T samples
     const int T = blockDim.x;
@@ -280,30 +278,8 @@ __global__ void __launch_bounds__(256) ar_inverse_kernel(const InvParams p) {
                 }
 #pragma unroll
                 for (int j = 0; j < R; ++j) {
-                    float xv, lj;
-                    if constexpr (UNI == ZK_UNI_RQS) {
-                        Bin b = rqs_select<KT, FAST, true>(phi[j], KT, yv[j], p.bound, p.aw, p.ad);
-                        xv = rqs_inverse_eval<FAST>(b, yv[j]);
-                        float y2;
-                        rqs_forward_eval<FAST>(b, xv, y2, lj);  // ladj of the forward map at the solution
-                        if (p.circ) xv = circ_shift(xv, p.bound);  // inverse of flows/spline.py:68-71
-                    } else if constexpr (UNI == ZK_UNI_SOSP) {
-                        xv = sosp::inverse<KT>(phi[j], p.sosp, yv[j]);
-                        lj = zlog<FAST>(sosp::g<KT>(phi[j], p.sosp, xv));  // ladj of the forward map at the solution
-                    } else if constexpr (UNI == ZK_UNI_BERNSTEIN) {
-                        constexpr int MT = bern::kDefM;
-                        float w[bern::kDefP], mx, rs;
-                        bern::softmax<bern::kDefP>(phi[j], p.bern, w, mx, rs);
-                        auto dl = [&](int q) { return bern::delta<bern::kDefP>(phi[j], w, p.bern, mx, rs, q); };
-                        xv = bern::inverse<MT>(p.bern, yv[j], dl);
-                        float fp;
-                        bern::forward<MT>(p.bern, xv, dl, &fp);
-                        lj = zlog<FAST>(fp);  // ladj of the forward map at the solution
-                    } else {
-                        const float ls = softclip<FAST>(phi[j][1], p.ad);
-                        xv = zdiv<FAST>(yv[j] - phi[j][0], zexp<FAST>(ls));
-                        lj = ls;
-                    }
+                    float lj;
+                    const float xv = UniFamily<UNI>::template inverse_ladj<KT, FAST>(phi[j], p, yv[j], lj);
                     lj *= p.sign;
                     if (p.base) {
                         const float u = ((p.base == 2 ? xv : yv[j]) - mu) * isg;
@@ -325,29 +301,6 @@ __global__ void __launch_bounds__(256) ar_inverse_kernel(const InvParams p) {
     }
 }
 
-template <int UNI, int KT>
-zk_status launch_inv_t(const InvParams& p, bool fast, int R, int grid, int T, size_t smem, cudaStream_t st) {
-    auto go = [&](auto kern) -> zk_status {
-        ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, T, smem, st>>>(p);
-        return check_launch("ar_inverse_kernel");
-    };
-    constexpr bool kTwo = UNI != ZK_UNI_SOSP && UNI != ZK_UNI_BERNSTEIN;  // bisections: one sample per thread only (inv_geometry)
-    if (p.act != 1) {  // general activation: one instantiation per sample tiling (IEEE math in the activation)
-        if constexpr (kTwo)
-            if (R == 2) return fast ? go(ar_inverse_kernel<UNI, KT, true, 2, true>) : go(ar_inverse_kernel<UNI, KT, false, 2, true>);
-        return fast ? go(ar_inverse_kernel<UNI, KT, true, 1, true>) : go(ar_inverse_kernel<UNI, KT, false, 1, true>);
-    }
-    if constexpr (kTwo) {
-        if (R == 2) {
-            if (fast) return go(ar_inverse_kernel<UNI, KT, true, 2, false>);
-            return go(ar_inverse_kernel<UNI, KT, false, 2, false>);
-        }
-    }
-    if (fast) return go(ar_inverse_kernel<UNI, KT, true, 1, false>);
-    return go(ar_inverse_kernel<UNI, KT, false, 1, false>);
-}
-
 // threads per CTA, samples per thread and shared memory for a pack.  ZK_INV_GEOM=TxR overrides the
 // choice (experiments); the default has not been re-tuned since the port to sm_90a.
 bool inv_geometry(const ArInvPack* pk, int* threads, int* per_thread, size_t* smem) {
@@ -358,7 +311,7 @@ bool inv_geometry(const ArInvPack* pk, int* threads, int* per_thread, size_t* sm
     auto set = [&](int T, int R) { *threads = T; *per_thread = R; *smem = per_sample * T * R + wbytes; return true; };
     if (const char* e = getenv("ZK_INV_GEOM")) {
         int T = 0, R = 0;
-        const bool r2 = pk->uni != ZK_UNI_SOSP && pk->uni != ZK_UNI_BERNSTEIN;  // R = 2 would spill (two register bisections); not compiled
+        const bool r2 = with_family(pk->uni, [](auto fam) { return decltype(fam)::kTwoPerThread; });  // else not compiled
         if (sscanf(e, "%dx%d", &T, &R) == 2 && (R == 1 || (R == 2 && r2)) && T >= 32 && T <= 256 && T % 32 == 0 && fits(T, R)) return set(T, R);
     }
     // two CTAs of 128 samples per SM when they fit (8 warps hide the FMA / LDS latencies of the dot
@@ -380,17 +333,15 @@ void ar_inverse_free(ArInvPack* pk) {
 }
 
 zk_status ar_inverse_pack(const zk_mlp* m, const uint8_t* const* mask_dev, const int64_t* order, int D, int C,
-                          int uni, int bins, int degree, int passes, ArInvPack** out) {
+                          const UniSpec& spec, int passes, ArInvPack** out) {
     *out = nullptr;
     const int L = m->n_linear;
     if (!order || L < 1 || L > 7) return ZK_OK;
     if (!m->plain) return ZK_OK;  // residual blocks use the sweeps
-    if (uni == ZK_UNI_RQS && bins != 8 && bins != 16) return ZK_OK;
-    if (uni == ZK_UNI_SOSP && (bins != sosp::kDefK || degree != sosp::kDefL)) return ZK_OK;  // compiled for P = 16 only
-    if (uni == ZK_UNI_BERNSTEIN && degree != bern::kDefDegree) return ZK_OK;  // compiled for P = 17 only
-    if (uni != ZK_UNI_RQS && uni != ZK_UNI_AFFINE && uni != ZK_UNI_SOSP && uni != ZK_UNI_BERNSTEIN) return ZK_OK;
+    const int kt = uni_kt<kSequential>(spec);
+    if (kt < 0) return ZK_OK;  // no compiled shape
     if (m->dims[0] != D + C) return ZK_OK;
-    const int P = uni_param_count(uni, bins, degree);
+    const int P = uni_P(spec);
     if (m->dims[L] != D * P) return ZK_OK;
     for (int d = 0; d < D; ++d)
         if (order[d] < 0 || order[d] >= passes) return ZK_OK;
@@ -428,7 +379,7 @@ zk_status ar_inverse_pack(const zk_mlp* m, const uint8_t* const* mask_dev, const
             if (ready[L - 1][d * P + q] > order[d]) return ZK_OK;  // not a pure order-class structure
 
     ArInvPack* pk = new ArInvPack();
-    pk->D = D; pk->C = C; pk->P = P; pk->uni = uni; pk->bins = bins; pk->degree = degree; pk->passes = passes; pk->n_linear = L;
+    pk->D = D; pk->C = C; pk->P = P; pk->uni = spec.kind; pk->kt = kt; pk->passes = passes; pk->n_linear = L;
     pk->act = m->act;
     pk->dims = m->dims;
     int off = 0;
@@ -584,30 +535,31 @@ zk_status launch_ar_inverse(const ArInvPack* pk, const ArInvArgs& a, cudaStream_
     p.sec_len[0] = pk->D + pk->C;
     for (int l = 1; l < pk->n_linear; ++l) p.sec_len[l] = pk->dims[l];
     p.y = a.y; p.ldy = a.ldy; p.c = a.c; p.ldc = a.ldc; p.x = a.x; p.ldx = a.ldx; p.B = a.B;
-    p.bound = a.bound;
-    p.circ = a.circular ? 1 : 0;
     p.act = pk->act;
-    const float absL = fabsf(logf(a.slope));
-    p.aw = 2.f / absL;
-    p.ad = 1.f / absL;
     p.ladj = a.ladj; p.accumulate = a.accumulate; p.base = a.base ? (a.as_inverse_member ? 2 : 1) : 0;
     p.sign = a.as_inverse_member ? -1.f : 1.f;
     p.base_loc = a.base_loc; p.base_scale = a.base_scale;
-    if (pk->uni == ZK_UNI_SOSP) p.sosp = sosp::make_const(pk->bins, pk->degree, a.bound, a.slope, a.iters);
     const int64_t grid = ceil_div(a.B, (int64_t)T * R);
     ZK_REQUIRE(grid <= 0x7fffffff, "ar_inverse: batch too large for one launch");
-    if (pk->uni == ZK_UNI_RQS && pk->bins == 8) return launch_inv_t<ZK_UNI_RQS, 8>(p, a.fast, R, (int)grid, T, smem, st);
-    if (pk->uni == ZK_UNI_RQS && pk->bins == 16) return launch_inv_t<ZK_UNI_RQS, 16>(p, a.fast, R, (int)grid, T, smem, st);
-    if (pk->uni == ZK_UNI_SOSP) {
-        ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "ar_inverse: bisection steps must be in [1, 64], got %d", a.iters);
-        return launch_inv_t<ZK_UNI_SOSP, sosp::kDefK>(p, a.fast, R, (int)grid, T, smem, st);
-    }
-    if (pk->uni == ZK_UNI_BERNSTEIN) {
-        ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "ar_inverse: bisection steps must be in [1, 64], got %d", a.iters);
-        p.bern = bern::make_const(pk->degree, a.bound, kBernsteinEps, a.iters);
-        return launch_inv_t<ZK_UNI_BERNSTEIN, bern::kDefP>(p, a.fast, R, (int)grid, T, smem, st);
-    }
-    return launch_inv_t<ZK_UNI_AFFINE, 0>(p, a.fast, R, (int)grid, T, smem, st);
+    ZK_TRY(uni_check_scalars(a.spec, true));
+    return uni_dispatch<kSequential>(pk->uni, pk->kt, a.fast, [&](auto fam, auto kt, auto fast) {
+        using Fam = decltype(fam);
+        set_uni_consts<Fam>(a.spec, p);
+        auto go = [&](auto kern) -> zk_status {
+            ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            kern<<<(int)grid, T, smem, st>>>(p);
+            return check_launch("ar_inverse_kernel");
+        };
+        // GACT: a general activation (IEEE math in the activation) instead of ReLU
+        auto tiled = [&](auto gact) {
+            constexpr int K = decltype(kt)::value;
+            constexpr bool F = decltype(fast)::value, G = decltype(gact)::value;
+            if constexpr (Fam::kTwoPerThread)
+                if (R == 2) return go(ar_inverse_kernel<Fam::kKind, K, F, 2, G>);
+            return go(ar_inverse_kernel<Fam::kKind, K, F, 1, G>);
+        };
+        return p.act != 1 ? tiled(std::true_type{}) : tiled(std::false_type{});
+    });
 }
 
 }  // namespace zk

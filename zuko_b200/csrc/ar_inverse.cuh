@@ -7,12 +7,12 @@ namespace zk {
 
 struct ArInvPack;  // step-ordered weight stream of one layer (ar_inverse.cu)
 
-// Builds the pack when the layer has a pure order-class structure (an `order` vector, RQS with 8 /
-// 16 bins, affine, SOSP with 3 polynomials of degree 4, or Bernstein of degree 16); leaves *out null (and returns ZK_OK) when
+// Builds the pack when the layer has a pure order-class structure (an `order` vector) and its bijector has a
+// compiled sequential-inverse shape (uni_kt<kSequential>); leaves *out null (and returns ZK_OK) when
 // the layer must use the generic sweep-based inverse instead.  `mask_dev` are the DEVICE mask pointers
 // of zk_mlp_desc (may be null).
 zk_status ar_inverse_pack(const zk_mlp* m, const uint8_t* const* mask_dev, const int64_t* order, int D, int C,
-                          int univariate, int bins, int degree, int passes, ArInvPack** out);
+                          const UniSpec& spec, int passes, ArInvPack** out);
 void ar_inverse_free(ArInvPack* pk);
 bool ar_inverse_threads(const ArInvPack* pk, int* threads, size_t* smem);
 // the launch geometry launch_ar_inverse uses (ZK_INV_GEOM honoured): threads per CTA, samples per
@@ -24,9 +24,8 @@ struct ArInvArgs {
     const float* c = nullptr; int64_t ldc = 0;
     int64_t B = 0;
     float* x = nullptr; int64_t ldx = 0;
-    float bound = 5.f, slope = 1e-3f;
-    int iters = 0;  // SOSP / Bernstein: bisection steps
-    bool fast = true, circular = false;
+    UniSpec spec;  // the one the pack was built for
+    bool fast = true;
     // optional: per-sample sum over D of the FORWARD log-derivative at the solution x (what
     // rsample_and_log_prob needs, distributions.py:129-138), accumulated into `ladj` when
     // `accumulate`; with `base` the DiagNormal(loc, scale) log-density of y is added as well

@@ -8,15 +8,11 @@
 
 #include "activations.cuh"
 #include "backward.cuh"
-#include "bijector_grad.cuh"
-#include "bijector_math.cuh"
+#include "uni_family.cuh"
 
 namespace zk {
 
-namespace {
-
-constexpr int kBwdThreads = 256;
-
+// outside the anonymous namespace: a family's Tables<UniBwdParams> derives from it
 struct UniBwdParams {
     const float* x; int64_t ldx;
     const float* phi; int64_t phi_ld;
@@ -30,28 +26,15 @@ struct UniBwdParams {
     int rows_per_tile;
     int circ;
 };
-// SOSP kernels also take the shape and the pre-scaled quadrature.  A type of their own: appending the
-// table to UniBwdParams changes the register allocation of the RQS and Gaussianization instantiations.
-struct SospBwdParams : UniBwdParams {
-    sosp::Const sosp;
-};
-// Bernstein kernels take the order, bound and eps the same way
-struct BernBwdParams : UniBwdParams {
-    bern::Const bern;
-};
-template <int UNI>
-struct BwdParamsFor { using type = UniBwdParams; };
-template <>
-struct BwdParamsFor<ZK_UNI_SOSP> { using type = SospBwdParams; };
-template <>
-struct BwdParamsFor<ZK_UNI_BERNSTEIN> { using type = BernBwdParams; };
 
-__device__ __forceinline__ float circ_shift_b(float x, float bound) {  // bijector_math.cuh:circ_shift
-    const float m = 2.f * bound;
-    float r = fmodf(x, m);
-    if (r != 0.f && r < 0.f) r += m;
-    return r - bound;
-}
+namespace {
+
+constexpr int kBwdThreads = 256;
+
+// A family with device tables gets them in a parameter type of its own (UniFamily::Tables): appending the tables
+// to UniBwdParams changes the register allocation of the instantiations that do not read them.
+template <class Fam>
+using BwdParams = typename Fam::template Tables<UniBwdParams>;
 
 // thread = (sample row, dim) pair; the tile's parameter block is staged in shared memory, every
 // pair rewrites its P slots with the parameter gradients, and the tile is written back with
@@ -59,7 +42,7 @@ __device__ __forceinline__ float circ_shift_b(float x, float bound) {  // biject
 // A shared table is rewritten in place too when the tile holds one row (uni_bwd_plan): pair d then
 // reads and writes only slots d*P.., and every CTA stages its own copy of the table.
 template <int UNI, int KT, bool FAST>
-__global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const typename BwdParamsFor<UNI>::type a) {
+__global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const BwdParams<UniFamily<UNI>> a) {
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x;
     const int64_t r0 = (int64_t)blockIdx.x * a.rows_per_tile;
@@ -84,39 +67,13 @@ __global__ void __launch_bounds__(kBwdThreads) uni_bwd_kernel(const typename Bwd
         const int d = p - row * D;
         const int col = a.dim_map ? a.dim_map[d] : d;
         float xv = a.x[(r0 + row) * a.ldx + col];
-        if (UNI == ZK_UNI_RQS && a.circ) xv = circ_shift_b(xv, a.bound);
+        if (UniFamily<UNI>::kCircular && a.circ) xv = bij::circ_shift(xv, a.bound);
         const float gyv = a.gy ? a.gy[(r0 + row) * a.ldgy + col] : 0.f;
         const float glv = a.gl ? a.gl[r0 + row] : 0.f;
         const float* pp = s_phi + (shared_tbl ? d * P : p * P);
         float* out = s_out + p * P;
         float gxv;
-        if constexpr (UNI == ZK_UNI_RQS) {
-            bijgrad::rqs_backward_pair<KT, FAST>(pp, a.K, xv, gyv, glv, a.bound, a.aw, a.ad, gxv, out);
-        } else if constexpr (UNI == ZK_UNI_GAUSS) {
-            float yv, lj;
-            bij::gauss_forward_eval<KT, FAST>(pp, a.K, xv, yv, lj);
-            bijgrad::gauss_backward_pair<FAST>(pp, KT > 0 ? KT : a.K, xv, yv, gyv, glv, gxv, out);
-        } else if constexpr (UNI == ZK_UNI_SOSP) {
-            if constexpr (KT > 0) {  // register copy of the parameters; out may alias pp
-                float ar[sosp::kDefP];
-#pragma unroll
-                for (int q = 0; q < sosp::kDefP; ++q) ar[q] = pp[q];
-                sosp::backward_pair<KT>(ar, a.sosp, xv, gyv, glv, gxv, out);
-            } else {
-                sosp::backward_pair<0>(pp, a.sosp, xv, gyv, glv, gxv, out);
-            }
-        } else if constexpr (UNI == ZK_UNI_BERNSTEIN) {
-            if constexpr (KT > 0) {  // register copy of the parameters; out may alias pp
-                float ur[bern::kDefP];
-#pragma unroll
-                for (int q = 0; q < bern::kDefP; ++q) ur[q] = pp[q];
-                bern::backward_pair<bern::kDefP>(ur, a.bern, xv, gyv, glv, gxv, out);
-            } else {
-                bern::backward_pair<0>(pp, a.bern, xv, gyv, glv, gxv, out);
-            }
-        } else {
-            bijgrad::affine_backward_pair(pp, xv, gyv, glv, a.ad, gxv, out);
-        }
+        UniFamily<UNI>::template backward<KT, FAST>(pp, a, xv, gyv, glv, gxv, out);
         if (a.gx) a.gx[(r0 + row) * a.ldgx + col] = gxv;
     }
     __syncthreads();
@@ -335,43 +292,15 @@ int wgrad_slices_max(int N, int K) {
     return (int)S;
 }
 
-template <int UNI, int KT>
-zk_status launch_uni_bwd_t(const typename BwdParamsFor<UNI>::type& p, bool fast, int grid, size_t smem, bool smem_attr,
-                           cudaStream_t st) {
-    auto go = [&](auto kern) -> zk_status {
-        if (smem_attr)
-            ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, kBwdThreads, smem, st>>>(p);
-        return check_launch("uni_bwd_kernel");
-    };
-    // affine: one expf per pair, not worth a variant; SOSP: no transcendental in its reverse mode;
-    // Bernstein: no approximated transcendental in its reverse mode
-    if (fast && UNI != ZK_UNI_AFFINE && UNI != ZK_UNI_SOSP && UNI != ZK_UNI_BERNSTEIN) return go(uni_bwd_kernel<UNI, KT, true>);
-    return go(uni_bwd_kernel<UNI, KT, false>);
-}
-
 }  // namespace
 
-zk_status uni_bwd_plan(int uni, int64_t B, int D, int K, int degree, int64_t phi_ld, UniBwdPlan& out) {
+zk_status uni_bwd_plan(const UniSpec& s, int64_t B, int D, int64_t phi_ld, UniBwdPlan& out) {
     ZK_REQUIRE(B >= 0 && D > 0, "univariate backward: bad shape B=%lld D=%d", (long long)B, D);
     out = UniBwdPlan{};
     if (B == 0) return ZK_OK;
-    ZK_REQUIRE(uni == ZK_UNI_AFFINE || uni == ZK_UNI_RQS || uni == ZK_UNI_GAUSS || uni == ZK_UNI_SOSP || uni == ZK_UNI_BERNSTEIN,
-               "univariate backward: unknown kind %d", uni);
-    if (uni == ZK_UNI_RQS) {
-        ZK_REQUIRE(K >= 1 && K <= 1024, "rqs backward: bins must be in [1, 1024], got %d", K);
-        out.kt = (K == 8 || K == 16) ? K : 0;
-    } else if (uni == ZK_UNI_GAUSS) {
-        ZK_REQUIRE(K >= 1 && K <= 1024, "gaussianization backward: components must be in [1, 1024], got %d", K);
-        out.kt = (K == 8 || K == 16) ? K : 0;
-    } else if (uni == ZK_UNI_SOSP) {
-        ZK_REQUIRE(sosp_shape_ok(K, degree), "sosp backward: polynomials %d / degree %d out of range", K, degree);
-        out.kt = (K == sosp::kDefK && degree == sosp::kDefL) ? sosp::kDefK : 0;
-    } else if (uni == ZK_UNI_BERNSTEIN) {
-        ZK_REQUIRE(bernstein_shape_ok(degree), "bernstein backward: degree must be in [0, 59], got %d", degree);
-        out.kt = (degree + 1 == bern::kDefP) ? bern::kDefP : 0;
-    }
-    const int P = uni_param_count(uni, K, degree);
+    ZK_TRY(uni_check_shape(s));
+    out.kt = uni_kt<kBackward>(s);
+    const int P = uni_P(s);
     ZK_REQUIRE(phi_ld == 0 || phi_ld >= (int64_t)D * P, "univariate backward: phi_ld too small");
 
     // tile = R rows: aim at >= 256 pairs and ~24 KB of phi per CTA, at most 96 KB with a shared table staged
@@ -400,55 +329,23 @@ zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream) {
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate backward: null input");
     UniBwdPlan plan;
-    ZK_TRY(uni_bwd_plan(a.univariate, a.B, a.D, a.K, a.degree, a.phi_ld, plan));
-    if (a.univariate == ZK_UNI_SOSP) {
-        ZK_REQUIRE(a.bound > 0.f, "sosp backward: bound must be positive");
-    } else if (a.univariate == ZK_UNI_BERNSTEIN) {
-        ZK_REQUIRE(a.bound > 0.f, "bernstein backward: bound must be positive");
-        ZK_REQUIRE(a.eps > 0.f && a.eps < 0.5f, "bernstein backward: eps must be in (0, 1/2), got %g", (double)a.eps);
-    }
-    ZK_REQUIRE(a.slope > 0.f && a.slope < 1.f, "univariate backward: slope must be in (0, 1)");
+    ZK_TRY(uni_bwd_plan(a.spec, a.B, a.D, a.phi_ld, plan));
+    ZK_TRY(uni_check_scalars(a.spec, false));
     ZK_REQUIRE(!(a.phi_ld == 0 && a.gphi == a.phi), "univariate backward: gphi cannot alias a shared table");
-    const int P = uni_param_count(a.univariate, a.K, a.degree);
-    UniBwdParams p;
-    p.x = a.x; p.ldx = a.ldx; p.phi = a.phi; p.phi_ld = a.phi_ld; p.gy = a.gy; p.ldgy = a.ldgy;
-    p.gl = a.gl; p.gx = a.gx; p.ldgx = a.ldgx; p.gphi = a.gphi; p.dim_map = a.dim_map; p.B = a.B;
-    p.D = a.D; p.K = a.K; p.P = P; p.bound = a.bound;
-    p.circ = (a.circular && a.univariate == ZK_UNI_RQS) ? 1 : 0;
-    const float absL = fabsf(logf(a.slope));
-    p.aw = 2.f / absL;
-    p.ad = 1.f / absL;
-    p.rows_per_tile = plan.rows_per_tile;
-    const int grid = plan.grid;
-    const size_t smem = plan.smem;
-    const bool attr = plan.smem_attr;
-    if (a.univariate == ZK_UNI_AFFINE) return launch_uni_bwd_t<ZK_UNI_AFFINE, 0>(p, a.fast_math, grid, smem, attr, stream);
-    if (a.univariate == ZK_UNI_GAUSS) {
-        switch (plan.kt) {
-            case 8: return launch_uni_bwd_t<ZK_UNI_GAUSS, 8>(p, a.fast_math, grid, smem, attr, stream);
-            case 16: return launch_uni_bwd_t<ZK_UNI_GAUSS, 16>(p, a.fast_math, grid, smem, attr, stream);
-            default: return launch_uni_bwd_t<ZK_UNI_GAUSS, 0>(p, a.fast_math, grid, smem, attr, stream);
-        }
-    }
-    if (a.univariate == ZK_UNI_SOSP) {
-        SospBwdParams sp;
-        static_cast<UniBwdParams&>(sp) = p;
-        sp.sosp = sosp::make_const(a.K, a.degree, a.bound, a.slope, 0);
-        if (plan.kt == sosp::kDefK) return launch_uni_bwd_t<ZK_UNI_SOSP, sosp::kDefK>(sp, a.fast_math, grid, smem, attr, stream);
-        return launch_uni_bwd_t<ZK_UNI_SOSP, 0>(sp, a.fast_math, grid, smem, attr, stream);
-    }
-    if (a.univariate == ZK_UNI_BERNSTEIN) {
-        BernBwdParams bp;
-        static_cast<UniBwdParams&>(bp) = p;
-        bp.bern = bern::make_const(a.degree, a.bound, a.eps, 0);
-        if (plan.kt == bern::kDefP) return launch_uni_bwd_t<ZK_UNI_BERNSTEIN, bern::kDefP>(bp, a.fast_math, grid, smem, attr, stream);
-        return launch_uni_bwd_t<ZK_UNI_BERNSTEIN, 0>(bp, a.fast_math, grid, smem, attr, stream);
-    }
-    switch (plan.kt) {
-        case 8: return launch_uni_bwd_t<ZK_UNI_RQS, 8>(p, a.fast_math, grid, smem, attr, stream);
-        case 16: return launch_uni_bwd_t<ZK_UNI_RQS, 16>(p, a.fast_math, grid, smem, attr, stream);
-        default: return launch_uni_bwd_t<ZK_UNI_RQS, 0>(p, a.fast_math, grid, smem, attr, stream);
-    }
+    return uni_dispatch<kBackward>(a.spec.kind, plan.kt, a.fast_math, [&](auto fam, auto kt, auto fast) {
+        using Fam = decltype(fam);
+        BwdParams<Fam> p;
+        p.x = a.x; p.ldx = a.ldx; p.phi = a.phi; p.phi_ld = a.phi_ld; p.gy = a.gy; p.ldgy = a.ldgy;
+        p.gl = a.gl; p.gx = a.gx; p.ldgx = a.ldgx; p.gphi = a.gphi; p.dim_map = a.dim_map; p.B = a.B;
+        p.D = a.D; p.K = a.spec.K; p.P = uni_P(a.spec);
+        p.rows_per_tile = plan.rows_per_tile;
+        set_uni_consts<Fam>(a.spec, p);
+        auto kern = uni_bwd_kernel<Fam::kKind, decltype(kt)::value, decltype(fast)::value>;
+        if (plan.smem_attr)
+            ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
+        kern<<<plan.grid, kBwdThreads, plan.smem, stream>>>(p);
+        return check_launch("uni_bwd_kernel");
+    });
 }
 
 zk_status launch_softclip_backward(const float* x, int64_t ldx, const float* gy, int64_t ldgy,

@@ -20,7 +20,7 @@ namespace zk {
 // per-sample parameter gradients (B, D*P) (may be phi itself when phi_ld == D*P); gx the direct
 // input gradient (column dim_map[d] like the forward pass).
 struct UniBwdArgs {
-    int univariate = ZK_UNI_RQS;
+    UniSpec spec;
     const float* x = nullptr; int64_t ldx = 0;
     const float* phi = nullptr; int64_t phi_ld = 0;  // 0 = shared (D, P) table
     const float* gy = nullptr; int64_t ldgy = 0;
@@ -29,12 +29,8 @@ struct UniBwdArgs {
     float* gphi = nullptr;  // (B, D*P) contiguous
     const int* dim_map = nullptr;
     int64_t B = 0;
-    int D = 0, K = 0;
-    int degree = 0;         // SOSP: polynomial degree L (K = polynomials); Bernstein: BPF degree
-    float eps = kBernsteinEps;  // Bernstein: branch threshold on t
-    float bound = 5.f, slope = 1e-3f;
-    bool circular = false;  // RQS: CircularShiftTransform(bound) in front (d shift / dx = 1)
-    bool fast_math = false; // MUFU reciprocal / ex2 in the RQS and Gaussianization pair math (zk_set_fast_math)
+    int D = 0;
+    bool fast_math = false; // MUFU reciprocal / ex2 where the family has a fast-math backward (zk_set_fast_math)
 };
 
 // Tile plan of uni_bwd_kernel (launch_univariate_backward and zk_univariate_backward_plan both take it from
@@ -45,10 +41,10 @@ struct UniBwdPlan {
     size_t smem = 0;              // dynamic shared memory: R rows, plus the shared table unless it is rewritten in place
     bool smem_attr = false;       // smem > 40 KB: the launch raises the dynamic shared memory attribute
     bool table_in_place = false;  // shared table and R = 1: the kernel writes the gradients over the staged table
-    int kt = 0;                   // compile-time shape: RQS 8 / 16, Gaussianization 8 / 16, SOSP 3, Bernstein 17; 0 = runtime
+    int kt = 0;                   // compile-time shape (uni_kt<kBackward>); 0 = runtime
 };
 // Validates the shape arguments as launch_univariate_backward does and fills `out`; B = 0 leaves it zero.  Host only.
-zk_status uni_bwd_plan(int uni, int64_t B, int D, int K, int degree, int64_t phi_ld, UniBwdPlan& out);
+zk_status uni_bwd_plan(const UniSpec& s, int64_t B, int D, int64_t phi_ld, UniBwdPlan& out);
 zk_status launch_univariate_backward(const UniBwdArgs& a, cudaStream_t stream);
 
 // gx = gy / (1 + t)^2 - 2 gl sign(x) / (bound (1 + t)), t = |x| / bound  (transforms.py:309-316)

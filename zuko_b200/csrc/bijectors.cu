@@ -2,16 +2,9 @@
 //
 // uni_kernel: one pass per flow layer over (B, D) with per-sample parameters
 //   phi (B, D, P):  x, phi  ->  y, sum_d log|dy/dx|  (+ optional DiagNormal log-prob)
-// replacing the ~95 eager aten ops of MonotonicRQSTransform.__init__ +
-// call_and_ladj + DependentTransform (zuko/transforms.py:469-490, 554-567, 210-214)
-// and the ~10 of MonotonicAffineTransform (zuko/transforms.py:426-446), and
-// GaussianizationTransform (zuko/transforms.py:834-875): K erfc terms and the closed-form
-// ladj instead of the reference's autograd call per forward (transforms.py:623-637), and its
-// bisection inverse (transforms.py:609-617, utils.py:159-183) run in registers, and the
-// sum-of-squares polynomial bijector of SOSPF (flows/polynomial.py:23-28, sosp_math.cuh): its
-// Gauss-Legendre forward, log g(x), and the same bisection on y - constant, and the bounded Bernstein
-// bijector of BPF (transforms.py:640-831, bernstein_math.cuh): softmax, the Bernstein sums, log f'(x),
-// and the bisection of the full map between its two linear branches.
+// for every univariate bijector family of uni_family.cuh (affine, RQS, Gaussianization, SOSP, Bernstein),
+// replacing the eager per-pair ops of the reference's transforms and DependentTransform's ladj sum
+// (zuko/transforms.py:210-214); the family's forward / inverse pair functions run in registers.
 //
 // Data movement: a CTA owns a tile of R consecutive sample rows.  With dense rows
 // (phi_ld = D*P) their phi block is one contiguous range of R*D*P floats in HBM; it is
@@ -28,8 +21,8 @@
 
 #include <math_constants.h>
 
-#include "bijector_math.cuh"
 #include "bijectors.cuh"
+#include "uni_family.cuh"
 
 namespace zk {
 
@@ -59,61 +52,10 @@ struct UniParams {
     bern::Const bern;  // Bernstein: order, bound, eps and bisection
 };
 
-// SOSP pair: the default shape works on a register copy of its 16 parameters (four 16-byte loads:
-// P = 16 puts every pair on the same banks, a 4-way rather than a 16-way conflict)
-template <int KT, bool INVERSE, bool FAST>
-__device__ __forceinline__ float sosp_pair(const float* pp, const sosp::Const& c, float xv, float& lj) {
-    auto run = [&](const float* ap) {
-        if constexpr (INVERSE) {
-            return sosp::inverse<KT>(ap, c, xv);
-        } else {
-            float gx;
-            const float yv = sosp::forward<KT>(ap, c, xv, gx);
-            lj = zlog<FAST>(gx);
-            return yv;
-        }
-    };
-    if constexpr (KT > 0) {
-        float ar[sosp::kDefP];
-#pragma unroll
-        for (int q = 0; q < sosp::kDefP / 4; ++q) {
-            const float4 v = reinterpret_cast<const float4*>(pp)[q];
-            ar[4 * q] = v.x; ar[4 * q + 1] = v.y; ar[4 * q + 2] = v.z; ar[4 * q + 3] = v.w;
-        }
-        return run(ar);
-    } else {
-        return run(pp);
-    }
-}
-
-// Bernstein pair: the default degree takes its 17 parameters to registers and keeps the scaled softmax
-// there; other degrees form each softmax entry from shared memory when the sums need it
-template <int KT, bool INVERSE, bool FAST>
-__device__ __forceinline__ float bern_pair(const float* pp, const bern::Const& c, float xv, float& lj) {
-    constexpr int PT = KT > 0 ? bern::kDefP : 0;
-    constexpr int MT = KT > 0 ? bern::kDefM : 0;
-    float u[PT > 0 ? PT : 1], w[PT > 0 ? PT : 1];
-    if constexpr (PT > 0) {
-#pragma unroll
-        for (int q = 0; q < PT; ++q) u[q] = pp[q];
-    }
-    const float* up = PT > 0 ? u : pp;
-    float mx, rs;
-    bern::softmax<PT>(up, c, w, mx, rs);
-    auto dl = [&](int j) { return bern::delta<PT>(up, w, c, mx, rs, j); };
-    if constexpr (INVERSE) {
-        return bern::inverse<MT>(c, xv, dl);
-    } else {
-        float fp;
-        const float yv = bern::forward<MT>(c, xv, dl, &fp);
-        lj = zlog<FAST>(fp);
-        return yv;
-    }
-}
-
-// UNI: ZK_UNI_*; KT: compile-time bins (0 = runtime K); INVERSE; FAST math
+// UNI: the family (uni_family.cuh); KT: compile-time shape (0 = runtime shape); INVERSE; FAST math
 template <int UNI, int KT, bool INVERSE, bool FAST>
 __global__ void __launch_bounds__(kUniThreads) uni_kernel(const UniParams a) {
+    using Fam = UniFamily<UNI>;
     extern __shared__ __align__(128) float smem[];
     __shared__ __align__(8) uint64_t bar;
 
@@ -167,36 +109,10 @@ __global__ void __launch_bounds__(kUniThreads) uni_kernel(const UniParams a) {
             float xv = a.x[(r0 + row) * a.ldx + col];
             const float* pp = s_phi + (shared_tbl ? d * P : p * P);
             float yv;
-            if constexpr (UNI == ZK_UNI_RQS) {
-                if constexpr (!INVERSE) {
-                    if (a.circ) xv = circ_shift(xv, a.bound);  // flows/spline.py:68-71
-                    Bin b = rqs_select<KT, FAST, false>(pp, a.K, xv, a.bound, a.aw, a.ad);
-                    rqs_forward_eval<FAST>(b, xv, yv, lj);
-                } else {
-                    Bin b = rqs_select<KT, FAST, true>(pp, a.K, xv, a.bound, a.aw, a.ad);
-                    yv = rqs_inverse_eval<FAST>(b, xv);
-                    if (a.circ) yv = circ_shift(yv, a.bound);
-                }
-            } else if constexpr (UNI == ZK_UNI_GAUSS) {
-                if constexpr (!INVERSE) {
-                    gauss_forward_eval<KT, FAST>(pp, a.K, xv, yv, lj);
-                } else {
-                    yv = gauss_inverse_eval<KT, FAST>(pp, a.K, xv, a.bound, a.iters);
-                }
-            } else if constexpr (UNI == ZK_UNI_SOSP) {
-                yv = sosp_pair<KT, INVERSE, FAST>(pp, a.sosp, xv, lj);
-            } else if constexpr (UNI == ZK_UNI_BERNSTEIN) {
-                yv = bern_pair<KT, INVERSE, FAST>(pp, a.bern, xv, lj);
-            } else {  // affine, transforms.py:435-446: phi = (shift, unconstrained log-scale)
-                const float shift = pp[0];
-                const float ls = softclip<FAST>(pp[1], a.ad);
-                if constexpr (!INVERSE) {
-                    yv = fmaf(xv, zexp<FAST>(ls), shift);
-                    lj = ls;
-                } else {
-                    yv = zdiv<FAST>(xv - shift, zexp<FAST>(ls));
-                }
-            }
+            if constexpr (!INVERSE)
+                yv = Fam::template forward<KT, FAST>(pp, a, xv, lj);
+            else
+                yv = Fam::template inverse<KT, FAST>(pp, a, xv);
             if (a.y) a.y[(r0 + row) * a.ldy + col] = yv;
             if (!INVERSE && a.log_prob) {
                 // DiagNormal.log_prob term of this dim (torch/distributions/normal.py:87-102)
@@ -234,69 +150,15 @@ __global__ void __launch_bounds__(kUniThreads) uni_kernel(const UniParams a) {
     }
 }
 
-template <int UNI, int KT, bool INVERSE>
-zk_status launch_uni_t(const UniParams& p, bool fast, int grid, size_t smem, bool smem_attr, cudaStream_t st) {
-    auto go = [&](auto kern) -> zk_status {
-        if (smem_attr)
-            ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, kUniThreads, smem, st>>>(p);
-        return check_launch("uni_kernel");
-    };
-    if (fast) return go(uni_kernel<UNI, KT, INVERSE, true>);
-    return go(uni_kernel<UNI, KT, INVERSE, false>);
-}
-
-// kt: the compile-time shape uni_plan picked (UniPlan::kt)
-template <bool INVERSE>
-zk_status launch_uni_dir(const UniParams& p, int uni, int kt, bool fast, int grid, size_t smem, bool smem_attr,
-                         cudaStream_t st) {
-    if (uni == ZK_UNI_AFFINE) return launch_uni_t<ZK_UNI_AFFINE, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
-    if (uni == ZK_UNI_GAUSS) {
-        switch (kt) {
-            case 8: return launch_uni_t<ZK_UNI_GAUSS, 8, INVERSE>(p, fast, grid, smem, smem_attr, st);
-            case 16: return launch_uni_t<ZK_UNI_GAUSS, 16, INVERSE>(p, fast, grid, smem, smem_attr, st);
-            default: return launch_uni_t<ZK_UNI_GAUSS, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
-        }
-    }
-    if (uni == ZK_UNI_SOSP) {
-        if (kt == sosp::kDefK) return launch_uni_t<ZK_UNI_SOSP, sosp::kDefK, INVERSE>(p, fast, grid, smem, smem_attr, st);
-        return launch_uni_t<ZK_UNI_SOSP, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
-    }
-    if (uni == ZK_UNI_BERNSTEIN) {
-        if (kt == bern::kDefP) return launch_uni_t<ZK_UNI_BERNSTEIN, bern::kDefP, INVERSE>(p, fast, grid, smem, smem_attr, st);
-        return launch_uni_t<ZK_UNI_BERNSTEIN, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
-    }
-    switch (kt) {
-        case 4: return launch_uni_t<ZK_UNI_RQS, 4, INVERSE>(p, fast, grid, smem, smem_attr, st);
-        case 8: return launch_uni_t<ZK_UNI_RQS, 8, INVERSE>(p, fast, grid, smem, smem_attr, st);
-        case 16: return launch_uni_t<ZK_UNI_RQS, 16, INVERSE>(p, fast, grid, smem, smem_attr, st);
-        default: return launch_uni_t<ZK_UNI_RQS, 0, INVERSE>(p, fast, grid, smem, smem_attr, st);
-    }
-}
-
 }  // namespace
 
-zk_status uni_plan(int uni, int64_t B, int D, int K, int degree, int64_t phi_ld, const float* phi, UniPlan& out) {
+zk_status uni_plan(const UniSpec& s, int64_t B, int D, int64_t phi_ld, const float* phi, UniPlan& out) {
     ZK_REQUIRE(B >= 0 && D > 0, "univariate: bad shape B=%lld D=%d", (long long)B, D);
     out = UniPlan{};
     if (B == 0) return ZK_OK;
-    ZK_REQUIRE(uni == ZK_UNI_AFFINE || uni == ZK_UNI_RQS || uni == ZK_UNI_GAUSS || uni == ZK_UNI_SOSP || uni == ZK_UNI_BERNSTEIN,
-               "univariate: unknown kind %d", uni);
-    if (uni == ZK_UNI_RQS) {
-        ZK_REQUIRE(K >= 1 && K <= 1024, "rqs: bins must be in [1, 1024], got %d", K);
-        out.kt = (K == 4 || K == 8 || K == 16) ? K : 0;
-    } else if (uni == ZK_UNI_GAUSS) {
-        ZK_REQUIRE(K >= 1 && K <= 1024, "gaussianization: components must be in [1, 1024], got %d", K);
-        out.kt = (K == 8 || K == 16) ? K : 0;
-    } else if (uni == ZK_UNI_SOSP) {
-        ZK_REQUIRE(sosp_shape_ok(K, degree), "sosp: polynomials %d / degree %d out of range (degree <= 15, K (degree + 1) + 1 <= 1024)",
-                   K, degree);
-        out.kt = (K == sosp::kDefK && degree == sosp::kDefL) ? sosp::kDefK : 0;
-    } else if (uni == ZK_UNI_BERNSTEIN) {
-        ZK_REQUIRE(bernstein_shape_ok(degree), "bernstein: degree must be in [0, 59], got %d", degree);
-        out.kt = (degree + 1 == bern::kDefP) ? bern::kDefP : 0;
-    }
-    const int P = uni_param_count(uni, K, degree);
+    ZK_TRY(uni_check_shape(s));
+    out.kt = uni_kt<kStandalone>(s);
+    const int P = uni_P(s);
     ZK_REQUIRE(phi_ld == 0 || phi_ld >= (int64_t)D * P, "univariate: phi_ld too small");
 
     // tile = R rows: aim at >= 256 pairs and ~24 KB of phi per CTA, bounded by shared memory
@@ -326,19 +188,8 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     if (a.B == 0) return ZK_OK;
     ZK_REQUIRE(a.x && a.phi, "univariate: null input");
     UniPlan plan;
-    ZK_TRY(uni_plan(a.univariate, a.B, a.D, a.K, a.degree, a.phi_ld, a.phi, plan));
-    if (a.univariate == ZK_UNI_GAUSS) {
-        ZK_REQUIRE(a.bound > 0.f, "gaussianization: bound must be positive");
-        if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "gaussianization: bisection steps must be in [1, 64], got %d", a.iters);
-    } else if (a.univariate == ZK_UNI_SOSP) {
-        ZK_REQUIRE(a.bound > 0.f, "sosp: bound must be positive");
-        if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "sosp: bisection steps must be in [1, 64], got %d", a.iters);
-    } else if (a.univariate == ZK_UNI_BERNSTEIN) {
-        ZK_REQUIRE(a.bound > 0.f, "bernstein: bound must be positive");
-        ZK_REQUIRE(a.eps > 0.f && a.eps < 0.5f, "bernstein: eps must be in (0, 1/2), got %g", (double)a.eps);
-        if (a.inverse) ZK_REQUIRE(a.iters >= 1 && a.iters <= 64, "bernstein: bisection steps must be in [1, 64], got %d", a.iters);
-    }
-    ZK_REQUIRE(a.slope > 0.f && a.slope < 1.f, "univariate: slope must be in (0, 1)");
+    ZK_TRY(uni_plan(a.spec, a.B, a.D, a.phi_ld, a.phi, plan));
+    ZK_TRY(uni_check_scalars(a.spec, a.inverse));
     if (a.inverse) ZK_REQUIRE(a.y != nullptr, "univariate inverse: null output");
     if (a.accumulate) ZK_REQUIRE(a.ladj != nullptr, "univariate: accumulate needs ladj");
 
@@ -346,20 +197,20 @@ zk_status launch_univariate(const UniArgs& a, cudaStream_t stream) {
     p.x = a.x; p.ldx = a.ldx; p.phi = a.phi; p.phi_ld = a.phi_ld;
     p.y = a.y; p.ldy = a.ldy; p.ladj = a.ladj; p.accumulate = a.accumulate;
     p.log_prob = a.log_prob; p.base_loc = a.base_loc; p.base_scale = a.base_scale;
-    p.dim_map = a.dim_map; p.B = a.B; p.D = a.D; p.K = a.K; p.P = uni_param_count(a.univariate, a.K, a.degree);
-    p.bound = a.bound;
-    p.circ = (a.circular && a.univariate == ZK_UNI_RQS) ? 1 : 0;
-    p.iters = a.iters;
-    if (a.univariate == ZK_UNI_SOSP) p.sosp = sosp::make_const(a.K, a.degree, a.bound, a.slope, a.iters);
-    if (a.univariate == ZK_UNI_BERNSTEIN) p.bern = bern::make_const(a.degree, a.bound, a.eps, a.iters);
-    const float absL = fabsf(logf(a.slope));
-    p.aw = 2.f / absL;
-    p.ad = 1.f / absL;
+    p.dim_map = a.dim_map; p.B = a.B; p.D = a.D; p.K = a.spec.K; p.P = uni_P(a.spec);
+    p.iters = a.spec.iters;
     p.rows_per_tile = plan.rows_per_tile;
     p.use_bulk = plan.bulk ? 1 : 0;
-    if (a.inverse)
-        return launch_uni_dir<true>(p, a.univariate, plan.kt, a.fast_math, plan.grid, plan.smem, plan.smem_attr, stream);
-    return launch_uni_dir<false>(p, a.univariate, plan.kt, a.fast_math, plan.grid, plan.smem, plan.smem_attr, stream);
+    return uni_dispatch<kStandalone>(a.spec.kind, plan.kt, a.fast_math, [&](auto fam, auto kt, auto fast) {
+        using Fam = decltype(fam);
+        set_uni_consts<Fam>(a.spec, p);
+        auto kern = a.inverse ? uni_kernel<Fam::kKind, decltype(kt)::value, true, decltype(fast)::value>
+                              : uni_kernel<Fam::kKind, decltype(kt)::value, false, decltype(fast)::value>;
+        if (plan.smem_attr)
+            ZK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
+        kern<<<plan.grid, kUniThreads, plan.smem, stream>>>(p);
+        return check_launch("uni_kernel");
+    });
 }
 
 // ---------------------------------------------------------------------------

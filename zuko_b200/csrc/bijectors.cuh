@@ -8,7 +8,7 @@ namespace zk {
 // One fused pass of a univariate bijector over a (B, D) batch with (B, D, P)
 // per-sample parameters (or one shared (D, P) table when phi_ld == 0).
 struct UniArgs {
-    int univariate = ZK_UNI_RQS;  // ZK_UNI_*
+    UniSpec spec;
     bool inverse = false;
     const float* x = nullptr;  // input (B, *) ; forward: x, inverse: y
     int64_t ldx = 0;
@@ -24,13 +24,6 @@ struct UniArgs {
     const int* dim_map = nullptr;  // (D) device: pair d lives in column dim_map[d] of x / y (coupling)
     int64_t B = 0;
     int D = 0;      // number of transformed dims (pairs per sample)
-    int K = 0;      // bins (RQS) / mixture components (Gaussianization) / polynomials (SOSP)
-    int degree = 0; // SOSP: polynomial degree L; Bernstein: BPF degree (P = degree + 1)
-    float bound = 5.f;
-    int iters = 0;  // Gaussianization / SOSP / Bernstein inverse: bisection steps on [-bound, bound]
-    float eps = kBernsteinEps;  // Bernstein: branch threshold on t = (x + bound) / 2 bound
-    float slope = 1e-3f;
-    bool circular = false;  // RQS only: CircularShiftTransform(bound) in front (forward) / behind (inverse)
     bool fast_math = true;  // MUFU rcp/ex2/lg2 fast path (default) vs IEEE div + expf/logf
 };
 
@@ -42,10 +35,10 @@ struct UniPlan {
     bool smem_attr = false;  // smem + the static barrier exceed the 48 KB default: raise the attribute
     bool bulk = false;       // cp.async.bulk for full tiles: dense rows, 16-byte aligned phi and tile
     bool shuffle = false;    // D <= 32 and a power of two: warp-shuffle ladj sum, else the fixed-order sum
-    int kt = 0;              // compile-time shape of the instantiation: RQS 4 / 8 / 16, GAUSS 8 / 16, SOSP 3, Bernstein 17
+    int kt = 0;              // compile-time shape of the instantiation (uni_kt<kStandalone>); 0 = runtime
 };
 // Validates the shape arguments as launch_univariate does and fills `out`; B = 0 leaves it zero.  Host only.
-zk_status uni_plan(int uni, int64_t B, int D, int K, int degree, int64_t phi_ld, const float* phi, UniPlan& out);
+zk_status uni_plan(const UniSpec& s, int64_t B, int D, int64_t phi_ld, const float* phi, UniPlan& out);
 zk_status launch_univariate(const UniArgs& a, cudaStream_t stream);
 
 zk_status launch_softclip(const float* x, int64_t ldx, int64_t B, int D, float bound, bool inverse,

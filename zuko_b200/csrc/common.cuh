@@ -50,26 +50,20 @@ inline zk_status check_launch(const char* what) {
 
 int sm_count();  // cached, current device
 
-// parameters per (sample, dim) pair of a univariate bijector (ZK_UNI_*; K = bins / components /
-// polynomials, degree: ZK_UNI_SOSP and ZK_UNI_BERNSTEIN only)
-inline int uni_param_count(int uni, int K, int degree) {
-    switch (uni) {
-        case ZK_UNI_RQS: return 3 * K - 1;
-        case ZK_UNI_GAUSS: return 2 * K;
-        case ZK_UNI_SOSP: return K * (degree + 1) + 1;
-        case ZK_UNI_BERNSTEIN: return degree + 1;
-        default: return 2;
-    }
-}
-// shape limits of the sum-of-squares polynomial bijector: degree <= 15 (16 quadrature nodes), P <= 1024
-inline bool sosp_shape_ok(int K, int degree) {
-    return K >= 1 && K <= 1023 && degree >= 0 && degree <= 15 && K * (degree + 1) + 1 <= 1024;
-}
-
-// shape limits of the bounded Bernstein bijector: order M = degree + 5 <= 64
-inline bool bernstein_shape_ok(int degree) { return degree >= 0 && degree <= 59; }
 // eps of BoundedBernsteinTransform in flow layers (zk_layer_desc carries no eps)
 constexpr float kBernsteinEps = 1e-6f;
+
+// A univariate bijector and its scalars (families: uni_family.cuh)
+struct UniSpec {
+    int kind = ZK_UNI_RQS;      // ZK_UNI_* (circular RQS: ZK_UNI_RQS with `circular`)
+    int K = 0;                  // bins (RQS) / mixture components (Gaussianization) / polynomials (SOSP)
+    int degree = 0;             // SOSP: polynomial degree L; Bernstein: BPF degree (P = degree + 1)
+    float bound = 5.f;          // spline bound, or the bisection interval [-bound, bound]
+    float slope = 1e-3f;
+    float eps = kBernsteinEps;  // Bernstein: branch threshold on t = (x + bound) / 2 bound
+    int iters = 0;              // Gaussianization / SOSP / Bernstein inverse: bisection steps
+    bool circular = false;      // RQS only: CircularShiftTransform(bound) in front (forward) / behind (inverse)
+};
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
