@@ -9,10 +9,11 @@
 //                        reader of an A operand is done with it, it is overwritten in place with the
 //                        layer's output (bias, activation, bf16 hi/lo split): activations never
 //                        leave shared memory;
-//        last layer    : its rows are regrouped so that a 64-row chunk holds whole dims; the
-//                        accumulators of a chunk (+ bias) are staged through shared memory and a
-//                        thread per (sample row, dim) evaluates the spline / affine bijector, the
-//                        log-derivative and the per-sample sum — phi never touches HBM.
+//        last layer    : its rows are regrouped so that a 64-row chunk holds whole dims, in a column
+//                        order (fused_out_chunk.cuh) that lets each thread gather one (sample row, dim)'s
+//                        parameters from its quad's accumulators with register shuffles; it evaluates
+//                        the spline / affine bijector, the log-derivative and the per-sample sum — phi
+//                        never touches HBM.
 //   HBM traffic per sample per layer: 4 (D + C) read + 4 (D + 1) written.
 //
 // Restates for one MaskedAutoregressiveTransform layer:  flows/autoregressive.py:207-215 (meta),
@@ -43,6 +44,7 @@
 
 #include "activations.cuh"
 #include "fused_common.cuh"
+#include "fused_out_chunk.cuh"
 
 namespace zk {
 
@@ -60,7 +62,8 @@ constexpr uint32_t F_TILE = FM * FK * 2;  // 8 KB: one plane of a 64 x 64 tile
 constexpr uint32_t F_STAGE = 2 * F_TILE;  // hi + lo
 constexpr uint32_t F_SMEM_MAX = 232448;   // 227 KB per block on sm_90
 
-// floats per row of the output-layer staging buffer: the chunk's DPC * P parameters, made odd (no bank conflicts)
+// floats per row of the output-layer staging region: the chunk's DPC * P parameters, made odd.  The region is still
+// allocated (it sizes the plan) but no longer used: output chunks are assembled in registers
 __host__ __device__ constexpr int f_srow(int dpc_p) { return dpc_p | 1; }
 
 struct FusedParams {
@@ -126,22 +129,22 @@ __global__ void __launch_bounds__(F_THREADS, 1)
 fused_layer_kernel(const __grid_constant__ FusedParams p) {
     using Cfg = LastCfg<UNI, KT>;
     constexpr int P = Cfg::P, DPC = Cfg::DPC, NL = Cfg::NL;
-    constexpr int NP = DPC * P, SROW = f_srow(NP);  // staged columns of an output chunk, staging row stride
+    constexpr int NP = DPC * P, SROW = f_srow(NP);  // parameters of an output chunk, row stride of the unused region
     constexpr bool WIDE = (ROWS == 128);
-    static_assert(NP <= NL && NL <= FK && NL % 8 == 0, "a last-layer chunk must fit its MMA width");
+    using Out = outchunk::Shape<P, DPC>;
+    static_assert(NP <= NL && NL <= FK && NL % 8 == 0 && Out::NCOL <= NL, "a last-layer chunk must fit its MMA width");
     static_assert(ROWS == 64 || ROWS == 128, "row tile: one or two wgmma M");
     const int n_terms = NT ? NT : p.n_terms;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    // [W ring: n_stages x 16 KB][A: ROWS / 64 x 2 planes x KBA x 8 KB][staging 2 x 64 x SROW fp32]
+    // [W ring: n_stages x 16 KB][A: ROWS / 64 x 2 planes x KBA x 8 KB][unused: 2 x 64 x SROW fp32]
     // [ladj partials 4 x ROWS][barriers]
     const int NS = p.n_stages;
     uint8_t* sW = smem;
     uint8_t* sA = smem + (size_t)NS * F_STAGE;
     const uint32_t a_plane = (uint32_t)p.KBA * F_TILE;
-    float* s_stage = (float*)(sA + (ROWS / FM) * 2 * (size_t)a_plane);
-    float* s_part = s_stage + 2 * FM * SROW;
+    float* s_part = (float*)(sA + (ROWS / FM) * 2 * (size_t)a_plane) + 2 * FM * SROW;
     uint64_t* full = (uint64_t*)(s_part + 4 * ROWS);         // [F_MAX_STAGES] TMA -> consumer
     uint64_t* empty = full + F_MAX_STAGES;                   // [F_MAX_STAGES] consumer -> TMA
     const int NR = WIDE ? NS : NS / 2;                       // slots per ring (64 rows: ring g = [g NR, g NR + NR))
@@ -197,7 +200,6 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
     const int w = tid >> 5, lane = tid & 31;
     uint8_t* myA = sA + (WIDE ? (size_t)cw * 2 * a_plane : 0);
     const uint32_t a_base = smem_u32(myA), w_base = smem_u32(sW);
-    float* stg = s_stage + cw * FM * SROW;
     float* part = s_part + (WIDE ? cw * 4 * FM : 0);  // [4][64]: partial (chunk parity, slot) of each row
     const int s0 = WIDE ? 0 : cw * NR;                // this warpgroup's ring
     int s = s0;
@@ -318,58 +320,48 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
             for (int q = 0; q < 4; ++q) {
                 const int ch = WIDE ? q : 2 * q + cw;
                 if (ch >= nch) continue;
+                // a warp's 16 x 16 blocks, one stmatrix.x4 per plane: matrix m holds rows 16 w + 8 (m & 1) ... and
+                // columns 8 (i0 + m / 2) ...; lane t addresses row t % 8 of matrix t / 8
 #pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int col = 8 * i + 2 * (lane & 3);
-                    const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + ch * FK + col));
+                for (int i0 = 0; i0 < 8; i0 += 2) {
+                    uint32_t hi[4], lo[4];
 #pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        const int r = w * 16 + (lane >> 2) + 8 * hh;
-                        float v[2] = {acc[q][4 * i + 2 * hh] + bb.x, acc[q][4 * i + 2 * hh + 1] + bb.y};
-                        if constexpr (GACT) {  // any ZK_ACT_* (nn.py:264-265)
-                            if constexpr (FAST) act_apply_n_fast<2>(v, p.act); else act_apply_n<2>(v, p.act);
-                        } else {
-                            v[0] = fmaxf(v[0], 0.f);
-                            v[1] = fmaxf(v[1], 0.f);
+                    for (int di = 0; di < 2; ++di) {
+                        const int i = i0 + di;
+                        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + ch * FK + 8 * i + 2 * (lane & 3)));
+#pragma unroll
+                        for (int hh = 0; hh < 2; ++hh) {
+                            float v[2] = {acc[q][4 * i + 2 * hh] + bb.x, acc[q][4 * i + 2 * hh + 1] + bb.y};
+                            if constexpr (GACT) {  // any ZK_ACT_* (nn.py:264-265)
+                                if constexpr (FAST) act_apply_n_fast<2>(v, p.act); else act_apply_n<2>(v, p.act);
+                            } else {
+                                v[0] = fmaxf(v[0], 0.f);
+                                v[1] = fmaxf(v[1], 0.f);
+                            }
+                            split2_bf16(v[0], v[1], hi[2 * di + hh], lo[2 * di + hh]);
                         }
-                        uint32_t hi, lo;
-                        split2_bf16(v[0], v[1], hi, lo);
-                        const uint32_t off = (uint32_t)ch * F_TILE + sw128_offset(r, col);
-                        *reinterpret_cast<uint32_t*>(myA + off) = hi;
-                        *reinterpret_cast<uint32_t*>(myA + a_plane + off) = lo;
                     }
+                    const uint32_t off = a_base + (uint32_t)ch * F_TILE +
+                                         sw128_offset(w * 16 + 8 * ((lane >> 3) & 1) + (lane & 7), 8 * (i0 + (lane >> 4)));
+                    stmatrix_x4(off, hi[0], hi[1], hi[2], hi[3]);
+                    stmatrix_x4(off + a_plane, lo[0], lo[1], lo[2], lo[3]);
                 }
             }
             fence_proxy_async();
             sync_a();
         }
 
-        // ---- last layer: chunk = whole dims -> staged raw parameters -> bijector + ladj per thread ----
-        const int r = tid & 63, slot = tid >> 6;  // evaluation: thread = (sample row, share of the chunk's dims)
+        // ---- last layer: chunk = whole dims -> parameters gathered from the quad's accumulators -> bijector + ladj ----
+        // evaluation: thread = (sample row, share of the chunk's dims), both within its quad's rows
+        const int r = w * 16 + outchunk::row(lane), slot = outchunk::slot(lane);
         const int64_t row = rb + r;
         const bool row_ok = row < p.M;
         const float* bias = p.bias[L - 1];
         // the bias pairs of output chunk ch that this thread adds to its accumulators
         auto load_bias = [&](float2 (&bb)[NL / 8], int ch) {
 #pragma unroll
-            for (int i = 0; i < NL / 8; ++i) {
-                if (8 * i >= NP) break;
+            for (int i = 0; i < NL / 8; ++i)
                 bb[i] = __ldg(reinterpret_cast<const float2*>(bias + ch * FK + 8 * i + 2 * (lane & 3)));
-            }
-        };
-        // accumulators + bias of output chunk ch -> this warpgroup's staging buffer
-        auto stage_chunk = [&](const float (&a)[NL / 2], const float2 (&bb)[NL / 8]) {
-#pragma unroll
-            for (int i = 0; i < NL / 8; ++i) {
-                if (8 * i >= NP) break;
-                const int col = 8 * i + 2 * (lane & 3);
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    float* dst = stg + (w * 16 + (lane >> 2) + 8 * hh) * SROW + col;
-                    if (col < NP) dst[0] = a[4 * i + 2 * hh] + bb[i].x;
-                    if (col + 1 < NP) dst[1] = a[4 * i + 2 * hh + 1] + bb[i].y;
-                }
-            }
         };
         // RQS: the input x of this thread's dim of output chunk ch (0 where the thread evaluates nothing)
         auto load_x = [&](int ch) -> float {
@@ -389,29 +381,36 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
             }
             ls += lj;
         };
-        // bijector + log-derivative of this thread's dims of staged chunk ch, summed into ls (RQS: xv = load_x(ch))
-        auto eval_chunk = [&](int ch, float& ls, float xv) {
-            const float* pr = stg + r * SROW;
+        // bijector + log-derivative of this thread's dims of output chunk ch, summed into ls, from the chunk's
+        // accumulators a and bias pairs bb (RQS: xv = load_x(ch)).  Every thread of the warpgroup calls it.
+        auto eval_chunk = [&](int ch, float& ls, float xv, float (&a)[NL / 2], const float2 (&bb)[NL / 8]) {
+#pragma unroll
+            for (int i = 0; i < NL / 8; ++i)
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    a[4 * i + 2 * hh] += bb[i].x;
+                    a[4 * i + 2 * hh + 1] += bb[i].y;
+                }
+            float pr[Out::NV];  // staging-order values NV * slot ... of row r
+            outchunk::assemble<P, DPC>(a, lane, [](float mine, int mask) { return __shfl_xor_sync(0xffffffffu, mine, mask); }, pr);
             if constexpr (UNI == ZK_UNI_RQS) {
                 if (slot < DPC) {
                     const int d = ch * DPC + slot;
                     if (d < p.D && row_ok) {
-                        float pp[P];
-#pragma unroll
-                        for (int j = 0; j < P; ++j) pp[j] = pr[slot * P + j];
                         float yv, lj;
-                        Bin b = rqs_select<KT, FAST, false>(pp, KT, xv, p.bound, p.aw, p.ad);
+                        Bin b = rqs_select<KT, FAST, false>(pr, KT, xv, p.bound, p.aw, p.ad);
                         rqs_forward_eval<FAST>(b, xv, yv, lj);
                         finish_dim(ls, d, yv, lj);
                     }
                 }
             } else {
                 static_assert(DPC == 32, "affine chunk layout: 32 (shift, log-scale) pairs");
+#pragma unroll
                 for (int j = 0; j < 16; ++j) {
-                    const int dl = slot * 16 + j, d = ch * DPC + dl;
+                    const int d = ch * DPC + slot * 16 + j;
                     if (d < p.D && row_ok) {
-                        const float shift = pr[2 * dl];
-                        const float ls_ = softclip<FAST>(pr[2 * dl + 1], p.ad);
+                        const float shift = pr[2 * j];
+                        const float ls_ = softclip<FAST>(pr[2 * j + 1], p.ad);
                         const float xv = __ldg(p.x + row * p.ldx + d);
                         finish_dim(ls, d, fmaf(xv, zexp<FAST>(ls_), shift), ls_);
                     }
@@ -456,10 +455,7 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                 wgmma_wait0();
                 acc_fence(acc);
                 for (int i = 0; i < hn; ++i) release((hs + i) % NS);
-                stage_chunk(acc, bb);
-                named_bar_sync(2 + cw, 128);
-                eval_chunk(ch, ls, xv);
-                named_bar_sync(2 + cw, 128);  // staging buffer free for the next chunk
+                eval_chunk(ch, ls, xv, acc, bb);
             };
             for (int ch = 0; ch < p.n_last; ch += 2) {
                 out_chunk(ch, ls0);
@@ -486,10 +482,7 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                 if (!mine) continue;
                 float2 bb[NL / 8];
                 load_bias(bb, ch);
-                stage_chunk(acc, bb);
-                named_bar_sync(2 + cw, 128);
-                eval_chunk(ch, lsum, load_x(ch));
-                named_bar_sync(2 + cw, 128);  // staging buffer free for the next chunk
+                eval_chunk(ch, lsum, load_x(ch), acc, bb);
             }
             part[(2 * cw + slot) * FM + r] = lsum;
         }
@@ -704,14 +697,11 @@ zk_status fused_layer_prepare(zk_mlp* m, const uint8_t* const* mask_dev, int uni
     }
     std::vector<std::vector<int>> perm;
     fused_degree_perm(m->dims.data(), L, Mk, perm);
-    // output layer: padded row ch * 64 + j holds parameter j % P of dim ch * DPC + j / P (or zeros)
+    // output layer: the 64 padded rows of chunk ch hold the P parameters of dims ch * DPC ... ch * DPC + DPC - 1 (or
+    // zeros), in the column order of fused_out_chunk.cuh
     f.n_last = (D + DPC - 1) / DPC;
-    std::vector<int> last_rows((size_t)f.n_last * FK, -1);
-    for (int ch = 0; ch < f.n_last; ++ch)
-        for (int j = 0; j < DPC * P; ++j) {
-            const int d = ch * DPC + j / P;
-            if (d < D) last_rows[(size_t)ch * FK + j] = d * P + j % P;
-        }
+    std::vector<int> last_rows((size_t)f.n_last * FK);
+    outchunk::last_rows(D, P, DPC, f.n_last, last_rows.data());
     // ---- device buffers ----
     for (auto* q : f.w) cudaFree(q);
     for (auto* q : f.bias) cudaFree(q);

@@ -127,6 +127,14 @@ __device__ __forceinline__ void wgmma_kblock(float (&d)[NA], uint32_t a_hi, uint
     }
 }
 
+// four 8 x 8 b16 matrices to shared memory: lane l gives the address of row l % 8 of matrix l / 8 (16 bytes), and
+// r[m] is the pair of matrix m at row l / 4, columns 2 (l % 4), 2 (l % 4) + 1 — an 8 x 8 block of the wgmma
+// accumulator fragment after packing to bf16x2
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+                 ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+
 // byte offset of K element k (< 64) of row r inside a 128B-swizzled tile of 128-byte rows
 __device__ __forceinline__ uint32_t sw128_offset(int r, int k) {
     return (uint32_t)r * 128u + ((((uint32_t)k >> 3) ^ ((uint32_t)r & 7u)) << 4) + (((uint32_t)k & 7u) << 1);
