@@ -233,6 +233,18 @@ def stream_ptr(device: torch.device) -> c_void_p:
     return c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def hold_storage(tensors) -> list:
+    """Detached aliases of the tensors a cache entry keyed on ``data_ptr`` was built from.  Kept with the entry,
+    they keep the storage alive, so that no other tensor can be allocated at the same address while the entry
+    exists: a fresh tensor (``_version`` 0) reusing the freed address of an earlier one — a new posterior draw
+    swapped in by ``torch.nn.utils.stateless``, say — would otherwise match the entry and be served stale.
+
+    Cost: each entry keeps one copy of the weights it was packed from alive until it is replaced — one per layer
+    handle, per stand-alone conditioner and per CNF, and up to 9 per autoregressive layer in its cache of
+    permutation-folded handles; for tensors a module still owns this is no extra memory."""
+    return [t.detach() for t in tensors if torch.is_tensor(t)]
+
+
 def require_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise EngineError(

@@ -240,14 +240,23 @@ class AcceleratedFlow(Flow):
         return super().forward(c)
 
 
-def accelerate(flow: nn.Module) -> AcceleratedFlow:
+def accelerate(flow: nn.Module) -> nn.Module:
     """Returns an engine-backed drop-in for ``flow`` (a reference ``zuko.lazy.Flow`` such as
     ``zuko.flows.NSF(...)``) that shares its parameters and buffers.
+
+    A reference ``zuko.bayesian.BayesianModel`` gives an engine :class:`~zuko_b200.bayesian.BayesianModel`
+    over ``accelerate(model.base)`` whose ``means`` / ``logvars`` are the reference's own.
 
     Move ``flow`` to its CUDA device first (or call ``.resync()`` / just call the result — buffer
     replacement is detected).  The engine is fp32-only: other parameter dtypes raise ``TypeError``
     (the reference's tests default to fp64, tests/conftest.py:12).
     """
+    if type(flow).__name__ == "BayesianModel":  # zuko/bayesian.py:48-100
+        from .bayesian import BayesianModel
+
+        model = BayesianModel(accelerate(flow.base), include_params=())  # no parameters, no draws
+        model.means, model.logvars = flow.means, flow.logvars
+        return model
     if not (hasattr(flow, "transform") and hasattr(flow, "base")):
         raise TypeError("accelerate() expects a lazy Flow (an object with .transform and .base)")
     for name, t in list(flow.named_parameters()) + list(flow.named_buffers()):

@@ -143,7 +143,8 @@ class OwnedLayer:
 
 class PackedLayerMixin:
     """Gives a lazy layer a cached ``zk_layer`` handle, rebuilt when any tensor it was
-    packed from changes (data pointer / version / device) — optimizer steps,
+    packed from changes (data pointer / version / device; the cache holds the storage it was packed from, so a
+    data pointer is never reused by another tensor while cached) — optimizer steps,
     ``load_state_dict``, ``.to()``, Bayesian re-parameterisation (zuko/bayesian.py:161-166)."""
 
     def _layer_tensors(self) -> list:
@@ -206,7 +207,7 @@ class PackedLayerMixin:
             with torch.cuda.device(dev):
                 E.check(E.lib().zk_layer_update_weights(ref.handle, W, Bv, E.stream_ptr(dev)))
             ref.generation += 1
-            self.__dict__["_zk_cache"] = (sig, ref)
+            self.__dict__["_zk_cache"] = (sig, ref, E.hold_storage(self._layer_tensors()))
             return ref
         self._zk_release()
         desc, keep = self._layer_desc()
@@ -222,7 +223,7 @@ class PackedLayerMixin:
             E.check(E.lib().zk_layer_create(ctypes.byref(desc), ctypes.byref(h)))
         del keep
         ref = OwnedLayer(h)
-        self.__dict__["_zk_cache"] = (sig, ref)
+        self.__dict__["_zk_cache"] = (sig, ref, E.hold_storage(self._layer_tensors()))
         return ref
 
     def _zk_layer(self) -> ctypes.c_void_p:

@@ -213,7 +213,7 @@ class MaskedAutoregressiveTransform(PackedLayerMixin, LazyTransform):
         ref = OwnedLayer(h)
         if len(cache) > 8:
             cache.clear()
-        cache[tuple(q)] = (sig, ref)
+        cache[tuple(q)] = (sig, ref, E.hold_storage(self._layer_tensors()))
         return ref
 
     def forward(self, c: Tensor | None = None) -> Transform:

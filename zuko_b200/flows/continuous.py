@@ -94,7 +94,7 @@ class FFJTransform(LazyTransform):
         E.check(E.lib().zk_cnf_create(ctypes.byref(desc), D, self.ode.in_features - D - 2 * F, F,
                                       freqs.data_ptr() if F else None, ctypes.byref(h)))  # fmt: skip
         del keep
-        self.__dict__["_zk_cnf"] = (sig, h)
+        self.__dict__["_zk_cnf"] = (sig, h, self.ode._held_storage() + E.hold_storage([fr]))
         return h
 
     def _release(self) -> None:

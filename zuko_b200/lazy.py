@@ -27,6 +27,7 @@ import torch.nn as nn
 from torch import Tensor
 from torch.distributions import Distribution, Transform
 
+from . import _engine as E
 from .distributions import NormalizingFlow
 from .transforms import ComposedTransform
 from .utils import Partial
@@ -122,7 +123,7 @@ class _Unconditional(Partial):
         if cached is not None and cached[0] == sig:
             return cached[1]
         obj = Partial.forward(self)
-        self.__dict__["_built"] = (sig, obj)
+        self.__dict__["_built"] = (sig, obj, E.hold_storage(list(self.args) + list(self.kwargs.values())))
         return obj
 
     def __getstate__(self):

@@ -158,6 +158,10 @@ class _EngineMLP(nn.Sequential):
                 sig.append(None if t is None else (t.data_ptr(), t._version, t.device, t.dtype))
         return tuple(sig)
 
+    def _held_storage(self) -> list:
+        """What a cache keyed on ``_signature()`` keeps alive with its entry (``_engine.hold_storage``)."""
+        return E.hold_storage([t for m in self._linears() for t in (m.weight, m.bias, getattr(m, "mask", None))])
+
     def mlp_desc(self, reindex=None) -> tuple[E.MlpDesc, list]:
         """Builds the ``zk_mlp_desc`` for the current parameters. Returns (desc, keepalive).
         ``reindex(i, n, weight, bias, mask)`` may substitute the tensors of linear layer ``i`` of ``n`` (used to
@@ -209,7 +213,7 @@ class _EngineMLP(nn.Sequential):
             finally:
                 E.lib().zk_set_pack_stream(None)
         del keep
-        self.__dict__["_zk_cache"] = (sig, h)
+        self.__dict__["_zk_cache"] = (sig, h, self._held_storage())
         return h
 
     def _release(self) -> None:
