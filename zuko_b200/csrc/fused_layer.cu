@@ -30,9 +30,10 @@
 //   slot in order, so its mbarrier phases can never be lapped.
 // 128-row tiles: warpgroup 1 owns rows 0-63 of the tile and warpgroup 2 rows 64-127, each with its own A
 //   operand; both multiply EVERY weight tile (one ring, two arrivals per slot, neither consumer skips a
-//   slot), so a tile brought in by TMA feeds 128 rows.  Hidden-layer MMAs are asynchronous (one group per tile,
-//   the next tile issued before waiting, a slot released one tile late); an output chunk's tiles are issued as
-//   one asynchronous batch that completes before its bijector runs.  The warpgroups only meet at the W ring.
+//   slot), so a tile brought in by TMA feeds 128 rows.  MMAs are asynchronous (one group per tile, the next tile
+//   issued before waiting, a slot released one tile late).  The output chunks go in pairs: a pair's tiles are one
+//   such stream that completes before the two chunks' bijectors run side by side.  The warpgroups only meet at the
+//   W ring.
 //   The producer runs on 40 registers and the consumers on 232 (setmaxnreg).
 
 #include <string.h>
@@ -371,19 +372,18 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
             }
             return 0.f;
         };
-        auto finish_dim = [&](float& ls, int d, float yv, float lj) {
-            if (p.y) p.y[row * p.ldy + d] = yv;
-            if (p.log_prob) {
-                const float mu = p.base_loc ? p.base_loc[d] : 0.f;
-                const float sg = p.base_scale ? p.base_scale[d] : 1.f;
-                const float u = (yv - mu) / sg;
-                lj += -0.5f * u * u - logf(sg) - kHalfLog2Pi;
-            }
-            ls += lj;
-        };
-        // bijector + log-derivative of this thread's dims of output chunk ch, summed into ls, from the chunk's
-        // accumulators a and bias pairs bb (RQS: xv = load_x(ch)).  Every thread of the warpgroup calls it.
-        auto eval_chunk = [&](int ch, float& ls, float xv, float (&a)[NL / 2], const float2 (&bb)[NL / 8]) {
+        // this thread's dims of output chunk ch: NE of them (RQS: one, affine: 16), dim j is d_of(ch, j); only those
+        // with keep(d) exist
+        constexpr int NE = (UNI == ZK_UNI_RQS) ? 1 : 16;
+        static_assert(UNI == ZK_UNI_RQS || DPC == 32, "affine chunk layout: 32 (shift, log-scale) pairs");
+        auto d_of = [&](int ch, int j) { return (UNI == ZK_UNI_RQS) ? ch * DPC + slot : ch * DPC + slot * 16 + j; };
+        auto keep = [&](int d) { return slot < DPC && d < p.D && row_ok; };
+        // value part: the bijector and log-derivative of this thread's dims of output chunk ch, from the chunk's
+        // accumulators a and bias pairs bb (RQS: xv = load_x(ch)).  Every thread of the warpgroup calls it, and it has
+        // no branch: a thread computes on whatever it holds, and store_chunk drops the dims that do not exist.  So the
+        // compiler can interleave two calls' dependent MUFU chains.
+        auto chunk_values = [&](int ch, float xv, float (&a)[NL / 2], const float2 (&bb)[NL / 8], float (&yv)[NE],
+                                float (&lj)[NE]) {
 #pragma unroll
             for (int i = 0; i < NL / 8; ++i)
 #pragma unroll
@@ -394,27 +394,34 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
             float pr[Out::NV];  // staging-order values NV * slot ... of row r
             outchunk::assemble<P, DPC>(a, lane, [](float mine, int mask) { return __shfl_xor_sync(0xffffffffu, mine, mask); }, pr);
             if constexpr (UNI == ZK_UNI_RQS) {
-                if (slot < DPC) {
-                    const int d = ch * DPC + slot;
-                    if (d < p.D && row_ok) {
-                        float yv, lj;
-                        Bin b = rqs_select<KT, FAST, false>(pr, KT, xv, p.bound, p.aw, p.ad);
-                        rqs_forward_eval<FAST>(b, xv, yv, lj);
-                        finish_dim(ls, d, yv, lj);
-                    }
-                }
+                Bin b = rqs_select<KT, FAST, false>(pr, KT, xv, p.bound, p.aw, p.ad);
+                rqs_forward_eval<FAST>(b, xv, yv[0], lj[0]);
             } else {
-                static_assert(DPC == 32, "affine chunk layout: 32 (shift, log-scale) pairs");
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int d = ch * DPC + slot * 16 + j;
-                    if (d < p.D && row_ok) {
-                        const float shift = pr[2 * j];
-                        const float ls_ = softclip<FAST>(pr[2 * j + 1], p.ad);
-                        const float xv = __ldg(p.x + row * p.ldx + d);
-                        finish_dim(ls, d, fmaf(xv, zexp<FAST>(ls_), shift), ls_);
-                    }
+                for (int j = 0; j < NE; ++j) {
+                    const int d = d_of(ch, j);
+                    const float x = keep(d) ? __ldg(p.x + row * p.ldx + d) : 0.f;
+                    lj[j] = softclip<FAST>(pr[2 * j + 1], p.ad);
+                    yv[j] = fmaf(x, zexp<FAST>(lj[j]), pr[2 * j]);
                 }
+            }
+        };
+        // store part: y of the dims that exist, and their log-derivatives (plus the base log-density on a flow's last
+        // layer) summed into ls.  The sum takes a select rather than a zero term, so that -0 partials keep their bits.
+        auto store_chunk = [&](int ch, float& ls, const float (&yv)[NE], const float (&lj)[NE]) {
+#pragma unroll
+            for (int j = 0; j < NE; ++j) {
+                const int d = d_of(ch, j);
+                const bool ok = keep(d);
+                if (ok && p.y) p.y[row * p.ldy + d] = yv[j];
+                float l = lj[j];
+                if (p.log_prob) {
+                    const float mu = (ok && p.base_loc) ? p.base_loc[d] : 0.f;
+                    const float sg = (ok && p.base_scale) ? p.base_scale[d] : 1.f;
+                    const float u = (yv[j] - mu) / sg;
+                    l += -0.5f * u * u - logf(sg) - kHalfLog2Pi;
+                }
+                ls = ok ? ls + l : ls;
             }
         };
         if constexpr (WIDE) {
@@ -427,39 +434,55 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                     for (int k = 0; k < len; k += 32) prefetch_l2(src + k);
                 }
             }
-            // a chunk's tiles (at most F_WIDE_MAXKB <= n_stages) are multiplied as one batch of asynchronous MMAs and
-            // released together once they are done.  The bijector runs with no MMAs in flight: its divergent
-            // branches inside a wgmma pipeline stage make ptxas serialize every wgmma of the kernel (C7515).  The
-            // chunk's bias and this thread's x are loaded before the batch is issued, so that their latency runs
-            // under the MMAs instead of after them.
-            float acc[NL / 2];
+            // The output chunks go in pairs (A, B) = (ch, ch + 1); with n_last odd the last pair's B is empty (no
+            // tiles, no dims).  A pair's tiles, A's then B's, are one stream of asynchronous MMAs with the hidden
+            // layers' discipline (one group per tile, a slot released once the next tile is issued), so B's tiles
+            // load and multiply behind A's and the pair ends in one full wait.  The bijector runs with no MMAs in
+            // flight: its code inside a wgmma pipeline stage makes ptxas serialize every wgmma of the kernel (C7515).
+            // Both chunks' bias and this thread's x are loaded before the pair's MMAs, so that their latency runs
+            // under the MMAs, and the two chunks' bijectors are evaluated side by side.
+            float accA[NL / 2], accB[NL / 2];
             float ls0 = 0.f, ls1 = 0.f;  // partials of the even and of the odd chunks
-            auto out_chunk = [&](int ch, float& ls) {
-#pragma unroll
-                for (int i = 0; i < NL / 2; ++i) acc[i] = 0.f;
-                float2 bb[NL / 8];
-                load_bias(bb, ch);
-                const float xv = load_x(ch);
-                const int hs = s;
-                int hn = 0;
-                for (int kb = 0; kb < nch; ++kb) {
-                    if (!((p.kbmask[L - 1][ch] >> kb) & 1u)) continue;
-                    mbar_wait(&full[s], ph);
-                    const uint32_t a_hi = a_base + (uint32_t)kb * F_TILE, w_tile = w_base + (uint32_t)s * F_STAGE;
-                    wgmma_fence();
-                    wgmma_kblock(acc, a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
-                    wgmma_commit();
-                    ++hn;
-                    advance();
-                }
-                wgmma_wait0();
-                acc_fence(acc);
-                for (int i = 0; i < hn; ++i) release((hs + i) % NS);
-                eval_chunk(ch, ls, xv, acc, bb);
-            };
             for (int ch = 0; ch < p.n_last; ch += 2) {
-                out_chunk(ch, ls0);
-                if (ch + 1 < p.n_last) out_chunk(ch + 1, ls1);
+                const bool has_b = ch + 1 < p.n_last;
+#pragma unroll
+                for (int i = 0; i < NL / 2; ++i) {
+                    accA[i] = 0.f;
+                    accB[i] = 0.f;
+                }
+                // B's zeros are set before A's MMAs: set inside that pipeline stage, they would serialize it (C7515)
+                acc_fence(accA);
+                acc_fence(accB);
+                float2 bbA[NL / 8], bbB[NL / 8];
+                load_bias(bbA, ch);
+                load_bias(bbB, ch + has_b);  // an empty B reads A's: its results are dropped
+                const float xA = load_x(ch), xB = load_x(ch + 1);
+                int held = -1;
+                auto issue = [&](float (&acc)[NL / 2], uint32_t kbmask) {
+                    for (int kb = 0; kb < nch; ++kb) {
+                        if (!((kbmask >> kb) & 1u)) continue;
+                        mbar_wait(&full[s], ph);
+                        const uint32_t a_hi = a_base + (uint32_t)kb * F_TILE, w_tile = w_base + (uint32_t)s * F_STAGE;
+                        wgmma_fence();
+                        wgmma_kblock(acc, a_hi, a_hi + a_plane, w_tile, w_tile + F_TILE, n_terms);
+                        wgmma_commit();
+                        wgmma_wait1();
+                        if (held >= 0) release(held);
+                        held = s;
+                        advance();
+                    }
+                };
+                issue(accA, p.kbmask[L - 1][ch]);
+                issue(accB, has_b ? p.kbmask[L - 1][ch + 1] : 0u);
+                wgmma_wait0();
+                if (held >= 0) release(held);
+                acc_fence(accA);
+                acc_fence(accB);
+                float yA[NE], ljA[NE], yB[NE], ljB[NE];
+                chunk_values(ch, xA, accA, bbA, yA, ljA);
+                chunk_values(ch + 1, xB, accB, bbB, yB, ljB);
+                store_chunk(ch, ls0, yA, ljA);
+                store_chunk(ch + 1, ls1, yB, ljB);
             }
             part[slot * FM + r] = ls0;
             part[(2 + slot) * FM + r] = ls1;
@@ -482,7 +505,9 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                 if (!mine) continue;
                 float2 bb[NL / 8];
                 load_bias(bb, ch);
-                eval_chunk(ch, lsum, load_x(ch), acc, bb);
+                float yv[NE], lj[NE];
+                chunk_values(ch, load_x(ch), acc, bb, yv, lj);
+                store_chunk(ch, lsum, yv, lj);
             }
             part[(2 * cw + slot) * FM + r] = lsum;
         }
