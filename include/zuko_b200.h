@@ -556,6 +556,64 @@ zk_status zk_cnf_backward(const zk_cnf* cnf, const float* x, int64_t ldx, const 
                           float* grad_c, int64_t ldgc, const zk_layer_grads* grads, void* workspace, size_t ws_bytes,
                           zk_stream stream);
 
+/* ------------------------------------------------------------------------- *
+ * Gaussian mixture model: GMM (zuko/mixtures.py:25-99) with Mixture.log_prob / sample
+ * (zuko/distributions.py:216-290).  A row's parameters phi come in the reference's unpack order
+ *     logits (K) | loc (K, D) | diag (L, Dd) | tril (L, D (D - 1) / 2)      L = tied ? 1 : K
+ * (Dd = 1 spherical, D otherwise; tril for ZK_COV_FULL only), zk_gmm_params_per_row() floats.  They are
+ * the conditioner's output rows hyper(c) when context > 0, else one caller-owned unconditional table `phi`
+ * read by every row.  Scale matrices: L_ii = exp(diag_i) + epsilon, tril below the diagonal in
+ * torch.tril_indices(D, D, -1) order; the per-row math is zuko_b200/csrc/gmm_math.cuh.
+ * Covered shapes: 1 <= features <= 64, 1 <= components <= 32; others are ZK_EUNSUPPORTED.
+ * Every call processes its batch in row chunks that fit the workspace (any workspace of at least
+ * zk_gmm_min_workspace_bytes() is accepted).
+ * ------------------------------------------------------------------------- */
+#define ZK_COV_FULL 0
+#define ZK_COV_DIAGONAL 1
+#define ZK_COV_SPHERICAL 2
+
+typedef struct {
+    int features, context, components, covariance, tied;
+    float epsilon;
+    const zk_mlp_desc* hyper; /* MLP(context -> params per row); NULL when context == 0 */
+} zk_gmm_desc;
+typedef struct zk_gmm zk_gmm;
+
+zk_status zk_gmm_create(const zk_gmm_desc* desc, zk_gmm** out);
+zk_status zk_gmm_destroy(zk_gmm* gmm);
+/* new conditioner weights / biases in place, as zk_layer_update_weights */
+zk_status zk_gmm_update_weights(zk_gmm* gmm, const float* const* weight, const float* const* bias, zk_stream stream);
+int64_t zk_gmm_params_per_row(int features, int components, int covariance, int tied);
+/* Launch plan of the mixture kernels (one thread per row, `threads` rows per CTA, per-row vectors in
+ * shared memory): threads, rows per CTA, dynamic shared memory of the log-density and of the backward
+ * kernel, and the instantiation (covariance * 2 + tied).  ZK_EUNSUPPORTED outside the covered shapes,
+ * ZK_EINVAL for an unknown covariance.  Outputs may be NULL.  No device work. */
+zk_status zk_gmm_plan(int features, int components, int covariance, int tied, int* threads, int* rows_per_cta,
+                      size_t* smem_log_prob, size_t* smem_backward, int* instantiated);
+/* workspace of log_prob / sample (resp. backward) processing B rows in one chunk; the minimum of any call */
+size_t zk_gmm_workspace_bytes(const zk_gmm* gmm, int64_t B);
+size_t zk_gmm_backward_workspace_bytes(const zk_gmm* gmm, int64_t B);
+size_t zk_gmm_min_workspace_bytes(const zk_gmm* gmm);
+/* rows of one chunk for this workspace (0 when it is below the minimum); backward != 0 for zk_gmm_backward */
+int64_t zk_gmm_chunk_rows(const zk_gmm* gmm, int64_t B, int backward, size_t ws_bytes);
+/* log_prob (B) of x (B, D); c (B, C) rows, or one broadcast row when ldc == 0 (NULL when C == 0);
+ * phi: the (params per row) table when C == 0, else NULL */
+zk_status zk_gmm_log_prob(const zk_gmm* gmm, const float* x, int64_t ldx, const float* c, int64_t ldc,
+                          const float* phi, int64_t B, float* log_prob, void* workspace, size_t ws_bytes,
+                          zk_stream stream);
+/* x (B, D) drawn from uniforms u (B) in [0, 1) (component) and standard normals z (B, D) */
+zk_status zk_gmm_sample(const zk_gmm* gmm, const float* c, int64_t ldc, const float* phi, const float* u,
+                        const float* z, int64_t ldz, int64_t B, float* x, int64_t ldx, void* workspace,
+                        size_t ws_bytes, zk_stream stream);
+/* Reverse mode of zk_gmm_log_prob for L = <grad_log_prob, log_prob>: writes grad_x (B, D) (may be NULL),
+ * ACCUMULATES grad_c ((B, C) rows, or one summed row when ldc == 0; may be NULL) and the parameter
+ * gradients: grads->grad_weight / grad_bias of the conditioner, or grads->grad_phi (params per row) of the
+ * unconditional table.  Sums over rows run in a fixed order: bit-identical run to run for one workspace. */
+zk_status zk_gmm_backward(const zk_gmm* gmm, const float* x, int64_t ldx, const float* c, int64_t ldc,
+                          const float* phi, int64_t B, const float* grad_log_prob, float* grad_x, int64_t ldgx,
+                          float* grad_c, int64_t ldgc, const zk_layer_grads* grads, void* workspace,
+                          size_t ws_bytes, zk_stream stream);
+
 /* 1 (default): the conditioner GEMMs of the backward pass (forward recompute, dgrad, wgrad) of a
  * handle packed for the tensor cores run on them (split-bf16, fp32 accumulate); 0: fp32 FMA on
  * CUDA cores (exact-order arbitration path).  Returns the previous value. */

@@ -9,7 +9,7 @@ The public surface mirrors the reference (probabilists/zuko) for the hot path on
 
 __version__ = "0.1.0"
 
-from . import bayesian, distributions, flows, lazy, nn, transforms, utils  # noqa: F401
+from . import bayesian, distributions, flows, lazy, mixtures, nn, transforms, utils  # noqa: F401
 from .accel import AcceleratedFlow, accelerate  # noqa: F401
 
 

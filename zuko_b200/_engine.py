@@ -35,6 +35,7 @@ ZK_GEMM_AUTO, ZK_GEMM_FP32, ZK_GEMM_BF16X3, ZK_GEMM_BF16X1 = range(4)
 (ZK_ACT_RELU, ZK_ACT_ELU, ZK_ACT_TANH, ZK_ACT_SILU, ZK_ACT_GELU, ZK_ACT_LEAKY_RELU, ZK_ACT_SOFTPLUS,
  ZK_ACT_SIGMOID) = (0, 2, 3, 4, 5, 6, 7, 8)  # fmt: skip
 ZK_CNF_TRACE_NONE, ZK_CNF_TRACE_EXACT, ZK_CNF_TRACE_HUTCHINSON = range(3)
+ZK_COV_FULL, ZK_COV_DIAGONAL, ZK_COV_SPHERICAL = range(3)
 GEMM_MODES = {"auto": ZK_GEMM_AUTO, "fp32": ZK_GEMM_FP32, "bf16x3": ZK_GEMM_BF16X3, "bf16x1": ZK_GEMM_BF16X1}
 
 
@@ -97,6 +98,18 @@ class FlowDesc(ctypes.Structure):
         ("base_scale", c_void_p),
         ("base_kind", c_int),
         ("inverted", POINTER(c_int)),
+    ]
+
+
+class GmmDesc(ctypes.Structure):
+    _fields_ = [
+        ("features", c_int),
+        ("context", c_int),
+        ("components", c_int),
+        ("covariance", c_int),
+        ("tied", c_int),
+        ("epsilon", c_float),
+        ("hyper", POINTER(MlpDesc)),
     ]
 
 
@@ -192,6 +205,20 @@ _SIGNATURES = {
     "zk_cnf_backward": (c_int, [_P, _P, c_int64, _P, c_int64, c_int64, _P, c_int, c_int, c_int, _P, c_int64, _P, c_int64, _P, _P,
                                 c_int64, _P, c_int64, POINTER(LayerGrads), _P, c_size_t, _P]),
     "zk_flow_log_prob_host": (c_int, [POINTER(FlowDesc), _P, c_int64, _P, c_int64, c_int64, _P, POINTER(c_double), _P, c_size_t, _P]),
+    "zk_gmm_create": (c_int, [POINTER(GmmDesc), POINTER(c_void_p)]),
+    "zk_gmm_destroy": (c_int, [_P]),
+    "zk_gmm_update_weights": (c_int, [_P, c_void_p, c_void_p, _P]),
+    "zk_gmm_params_per_row": (c_int64, [c_int, c_int, c_int, c_int]),
+    "zk_gmm_plan": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_size_t), POINTER(c_size_t),
+                            POINTER(c_int)]),
+    "zk_gmm_workspace_bytes": (c_size_t, [_P, c_int64]),
+    "zk_gmm_backward_workspace_bytes": (c_size_t, [_P, c_int64]),
+    "zk_gmm_min_workspace_bytes": (c_size_t, [_P]),
+    "zk_gmm_chunk_rows": (c_int64, [_P, c_int64, c_int, c_size_t]),
+    "zk_gmm_log_prob": (c_int, [_P, _P, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_size_t, _P]),
+    "zk_gmm_sample": (c_int, [_P, _P, c_int64, _P, _P, _P, c_int64, c_int64, _P, c_int64, _P, c_size_t, _P]),
+    "zk_gmm_backward": (c_int, [_P, _P, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64, _P, c_int64, POINTER(LayerGrads),
+                                _P, c_size_t, _P]),
 }  # fmt: skip
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -240,11 +240,30 @@ class AcceleratedFlow(Flow):
         return super().forward(c)
 
 
+def _accelerate_gmm(gmm: nn.Module) -> nn.Module:
+    """The engine's ``GMM`` on the reference model's own parameters (``hyper.*`` or ``phi.*``)."""
+    from .mixtures import GMM
+
+    for name, t in gmm.named_parameters():
+        if t.dtype != torch.float32:
+            raise TypeError(f"zuko_b200.accelerate: {name} is {t.dtype}; the engine computes in float32")
+    kwargs, context = {}, 0
+    if hasattr(gmm, "hyper"):
+        kwargs, linears = _conditioner_kwargs(gmm.hyper)
+        context = linears[0].weight.shape[1]
+    with torch.random.fork_rng(devices=[]):
+        mirror = GMM(gmm.shapes[1][1], context, components=gmm.components, covariance_type=gmm.covariance_type,
+                     tied=gmm.tied, epsilon=gmm.epsilon, **kwargs)  # fmt: skip
+    _share(mirror, gmm)
+    return mirror
+
+
 def accelerate(flow: nn.Module) -> nn.Module:
     """Returns an engine-backed drop-in for ``flow`` (a reference ``zuko.lazy.Flow`` such as
     ``zuko.flows.NSF(...)``) that shares its parameters and buffers.
 
-    A reference ``zuko.bayesian.BayesianModel`` gives an engine :class:`~zuko_b200.bayesian.BayesianModel`
+    A reference ``zuko.mixtures.GMM`` gives the engine's :class:`~zuko_b200.mixtures.GMM` on the reference's
+    own parameters.  A reference ``zuko.bayesian.BayesianModel`` gives an engine :class:`~zuko_b200.bayesian.BayesianModel`
     over ``accelerate(model.base)`` whose ``means`` / ``logvars`` are the reference's own.
 
     Move ``flow`` to its CUDA device first (or call ``.resync()`` / just call the result — buffer
@@ -257,6 +276,8 @@ def accelerate(flow: nn.Module) -> nn.Module:
         model = BayesianModel(accelerate(flow.base), include_params=())  # no parameters, no draws
         model.means, model.logvars = flow.means, flow.logvars
         return model
+    if type(flow).__name__ == "GMM":  # zuko/mixtures.py:25-99
+        return _accelerate_gmm(flow)
     if not (hasattr(flow, "transform") and hasattr(flow, "base")):
         raise TypeError("accelerate() expects a lazy Flow (an object with .transform and .base)")
     for name, t in list(flow.named_parameters()) + list(flow.named_buffers()):

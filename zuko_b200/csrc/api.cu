@@ -474,17 +474,7 @@ void zk_set_pack_stream(zk_stream stream) { g_pack_stream = (cudaStream_t)stream
 zk_status zk_layer_update_weights(zk_layer* l, const float* const* weight, const float* const* bias, zk_stream stream) {
     ZK_REQUIRE(l && weight, "layer_update_weights: null argument");
     ZK_REQUIRE(l->hyper, "layer_update_weights: the layer has no conditioner");
-    zk_mlp* m = l->hyper;
-    cudaStream_t st = (cudaStream_t)stream;
-    for (int i = 0; i < m->n_linear; ++i) {
-        ZK_REQUIRE(weight[i], "layer_update_weights: weight[%d] is null", i);
-        const int64_t n = (int64_t)m->dims[i + 1] * m->dims[i];
-        ZK_TRY(launch_apply_mask(weight[i], m->mask[i], n, m->w[i], st));  // nn.py:218 `mask * W`, once per update
-        if (bias && bias[i]) ZK_CUDA(cudaMemcpyAsync(m->b[i], bias[i], (size_t)m->dims[i + 1] * 4, cudaMemcpyDeviceToDevice, st));
-    }
-    ZK_TRY(tc_refresh(m, st));
-    ZK_TRY(fused_refresh(m, st));
-    m->bwd_dirty = true;          // transposed weights / backward planes: refilled by the next backward call
+    ZK_TRY(mlp_update_weights(l->hyper, weight, bias, (cudaStream_t)stream));
     if (l->inv) l->inv_dirty = true;  // step-ordered inverse stream: rebuilt by the next inverse call
     return ZK_OK;
 }
@@ -555,6 +545,19 @@ size_t zk_layer_workspace_bytes(const zk_layer* l, int64_t B) {
 }  // extern "C"
 
 namespace zkapi {
+
+zk_status mlp_update_weights(zk_mlp* m, const float* const* weight, const float* const* bias, cudaStream_t st) {
+    for (int i = 0; i < m->n_linear; ++i) {
+        ZK_REQUIRE(weight[i], "layer_update_weights: weight[%d] is null", i);
+        const int64_t n = (int64_t)m->dims[i + 1] * m->dims[i];
+        ZK_TRY(launch_apply_mask(weight[i], m->mask[i], n, m->w[i], st));  // nn.py:218 `mask * W`, once per update
+        if (bias && bias[i]) ZK_CUDA(cudaMemcpyAsync(m->b[i], bias[i], (size_t)m->dims[i + 1] * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    ZK_TRY(tc_refresh(m, st));
+    ZK_TRY(fused_refresh(m, st));
+    m->bwd_dirty = true;  // transposed weights / backward planes: refilled by the next backward call
+    return ZK_OK;
+}
 
 // gather of the constant split: xa[:, j] = x[:, idx_a[j]] (transforms.py:1040-1041)
 __global__ void gather_columns_kernel(const float* x, int64_t ldx, const int* cols, int n, int64_t B,

@@ -29,6 +29,10 @@ namespace {
 std::mutex g_bwd_mu;
 std::atomic<int> g_tc_backward{1};
 
+}  // namespace
+
+bool tc_backward_on() { return g_tc_backward.load() != 0; }
+
 // transposed pre-masked weights for dgrad, built on first use
 zk_status mlp_ensure_backward(const zk_mlp* cm, cudaStream_t st) {
     zk_mlp* m = const_cast<zk_mlp*>(cm);
@@ -53,15 +57,6 @@ zk_status mlp_ensure_backward(const zk_mlp* cm, cudaStream_t st) {
     ZK_CUDA(cudaStreamSynchronize(st));
     return ZK_OK;
 }
-
-struct MlpBwdBufs {
-    std::vector<float*> acts;  // acts[i]: input of linear layer i, (B, dims[i])
-    std::vector<float*> pre;   // pre[i]: pre-activation of hidden layer i + 1 (non-ReLU activations only)
-    float* out = nullptr;      // (B, dims[n]): conditioner output, later its gradient
-    float* gbuf[2] = {nullptr, nullptr};
-    float* gin = nullptr;      // (B, dims[0])
-    void* scratch = nullptr;
-};
 
 size_t mlp_bwd_scratch(const zk_mlp* m) {
     size_t s = colsum_scratch_bytes(m->dims[0]);  // broadcast-context column sum of the input gradient
@@ -152,14 +147,6 @@ zk_status mlp_backward(const zk_mlp* m, const MlpBwdBufs& b, int64_t B, bool wan
 // forward recompute with saved activations, dgrad, wgrad — is linear_tc_kernel (split-bf16, fp32
 // accumulation); see the block comment at the end of mlp_tcgen05.cu.
 // ---------------------------------------------------------------------------
-struct TcBwdPlan {
-    int n = 0;
-    std::vector<int> Kp;       // pad64(dims[i]), i = 0..n
-    std::vector<int> S, Bs, slice_m;  // per linear layer: batch slices of the wgrad GEMM
-    int max_hidden_kp = 0;
-    size_t gT = 0, aT = 0, partial = 0, scratch = 0;
-};
-
 TcBwdPlan tc_plan(const zk_mlp* m, int64_t B) {
     TcBwdPlan p;
     p.n = m->n_linear;
@@ -197,19 +184,6 @@ size_t tc_bwd_ws(const zk_mlp* m, int64_t B) {
     if (p.n > 1) s += 2 * a256((size_t)B * p.max_hidden_kp * 4);        // dgrad ping-pong planes
     return s + a256(p.gT) + a256(p.aT) + a256(p.partial) + a256(p.scratch);
 }
-
-struct TcBwdBufs {
-    float* a0 = nullptr;
-    float* gin = nullptr;
-    std::vector<__nv_bfloat16*> P;  // saved activation planes, [2][B][Kp[i]]
-    float* out = nullptr;           // phi, then gphi
-    __nv_bfloat16* G = nullptr;     // planes of gphi
-    __nv_bfloat16* gbuf[2] = {nullptr, nullptr};
-    __nv_bfloat16* gT = nullptr;
-    __nv_bfloat16* aT = nullptr;
-    float* partial = nullptr;
-    void* scratch = nullptr;
-};
 
 bool tc_bwd_carve(const zk_mlp* m, const TcBwdPlan& p, int64_t B, Arena& ar, TcBwdBufs& b) {
     b.a0 = ar.take<float>((size_t)B * m->dims[0]);
@@ -282,6 +256,8 @@ zk_status tc_mlp_backward(const zk_mlp* m, const TcBwdPlan& p, const TcBwdBufs& 
     }
     return ZK_OK;
 }
+
+namespace {
 
 size_t layer_bwd_ws(const zk_layer* l, int64_t B) {
     if (!l || B <= 0) return 0;

@@ -1,19 +1,22 @@
-"""Distributions of the flow hot path: ``NormalizingFlow`` and ``DiagNormal``.
+"""Distributions of the hot path: ``NormalizingFlow``, ``DiagNormal`` and the Gaussian ``Mixture``.
 
-Host-side mirror of zuko/distributions.py:39-138 (NormalizingFlow) and :337-363
+Host-side mirror of zuko/distributions.py:39-138 (NormalizingFlow), :216-290 (Mixture) and :337-363
 (DiagNormal).  Densities and inverse passes run in the H100 engine; torch provides the
 random numbers (``torch.randn`` on the device) and owns all memory.
 """
 
 from __future__ import annotations
 
-__all__ = ["BoxUniform", "DiagNormal", "NormalizingFlow"]
+__all__ = ["BoxUniform", "DiagNormal", "Mixture", "NormalizingFlow"]
 
 from textwrap import indent
 
+import ctypes
+from math import prod
+
 import torch
 from torch import Size, Tensor
-from torch.distributions import Distribution, Transform, constraints
+from torch.distributions import Distribution, Independent, MultivariateNormal, Normal, Transform, constraints
 
 from . import _engine as E
 from . import _ops
@@ -274,3 +277,201 @@ class NormalizingFlow(Distribution):
         if self.reinterpreted:
             ladj = ladj.sum(dim=tuple(range(-self.reinterpreted, 0)))
         return x, self.base.log_prob(z) - ladj
+
+
+class _GMMCall:
+    """The components of ``GMM(c)``: the model and its context (``None`` when unconditional).  The
+    base a :class:`Mixture` is built over."""
+
+    def __init__(self, gmm, c: Tensor | None) -> None:  # noqa: ANN001
+        self.gmm, self.c = gmm, c
+        self.batch_shape = Size(()) if c is None else c.shape[:-1]
+
+    def phi(self) -> tuple[Tensor, ...]:
+        """The parameter tensors with the reference's shapes, detached (inspection only)."""
+        from .utils import unpack
+
+        gmm = self.gmm
+        if self.c is None:
+            return tuple(p.detach() for p in gmm.phi)
+        with torch.no_grad():
+            return unpack(gmm.hyper(self.c), gmm.shapes)
+
+
+class Mixture(Distribution):
+    r"""Mixture of Gaussian components (zuko/distributions.py:216-290), built by :class:`zuko_b200.mixtures.GMM`.
+
+    .. math:: p(X = x) = \frac{1}{\sum_i w_i} \sum_i w_i \, p(Z_i = x)
+
+    ``log_prob`` is one engine call (``zk_gmm_log_prob``) behind an autograd function whose backward is
+    one ``zk_gmm_backward`` call: gradients reach ``x``, the context (reduced to its own shape) and every
+    parameter of the model.  ``sample(shape)`` draws ``u = torch.rand(n)`` then ``z = torch.randn(n, D)``
+    on the device and makes one ``zk_gmm_sample`` call.  As in the reference there is no ``rsample``.
+
+    ``logits`` and ``base`` (a ``MultivariateNormal``, or an ``Independent(Normal)`` for diagonal and
+    spherical covariances) are materialised on access, detached, with the reference's shapes: they are
+    for inspection and carry no gradient.  Only the components of a ``GMM`` are accepted as base.
+    """
+
+    has_rsample = False
+    arg_constraints = {}
+
+    def __init__(self, base: _GMMCall, logits: Tensor | None = None) -> None:
+        if not isinstance(base, _GMMCall) or logits is not None:
+            raise NotImplementedError("zuko_b200: Mixture is implemented for the components of zuko_b200.mixtures.GMM only")
+        self._call = base
+        self._batch = base.batch_shape
+        super().__init__(validate_args=False)
+
+    def __repr__(self) -> str:
+        return f"{self.__class__.__name__}({self.base})"
+
+    @property
+    def batch_shape(self) -> Size:
+        return self._batch
+
+    @property
+    def event_shape(self) -> Size:
+        return Size((self._call.gmm.features,))
+
+    @property
+    def support(self) -> constraints.Constraint:
+        return constraints.real_vector
+
+    def expand(self, batch_shape: Size, new: Distribution | None = None) -> Distribution:
+        new = self._get_checked_instance(Mixture, new)
+        new._call = self._call
+        new._batch = Size(batch_shape)
+        Distribution.__init__(new, validate_args=False)
+        return new
+
+    @property
+    def logits(self) -> Tensor:
+        logits = self._call.phi()[0]
+        return logits.expand(*self._batch, logits.shape[-1])
+
+    @property
+    def base(self) -> Distribution:
+        gmm = self._call.gmm
+        phi = self._call.phi()
+        K, D = gmm.components, gmm.features
+        loc = phi[1].expand(*self._batch, K, D)
+        scale = phi[2].exp() + gmm.epsilon
+        if gmm.covariance_type == "full":
+            tril = torch.diag_embed(scale)
+            mask = torch.tril(torch.ones_like(tril, dtype=bool), diagonal=-1)
+            tril = torch.masked_scatter(tril, mask, phi[3])
+            return MultivariateNormal(loc=loc, scale_tril=tril.expand(*self._batch, K, D, D))
+        return Independent(Normal(loc, scale.expand(*self._batch, K, D)), 1)
+
+    def _rows(self, lead: Size) -> tuple[Tensor | None, int]:
+        """The context as engine rows for the batch ``lead``: (c (n, C), ldc), one broadcast row (ldc = 0)
+        for a context without batch dimensions, ``(None, 0)`` when unconditional."""
+        c = self._call.c
+        if c is None:
+            return None, 0
+        E.require_cuda(c, "context")
+        if c.dim() == 1:
+            return c.contiguous(), 0
+        C = c.shape[-1]
+        return c.expand(*lead, C).reshape(-1, C).contiguous(), C
+
+    def log_prob(self, x: Tensor) -> Tensor:
+        E.require_cuda(x, "input")
+        gmm = self._call.gmm
+        D = gmm.features
+        lead = torch.broadcast_shapes(x.shape[:-1], self._batch)
+        x2 = x.expand(*lead, D).reshape(-1, D).contiguous()
+        c2, ldc = self._rows(lead)
+        return _MixtureLogProb.apply(gmm, ldc, x2, c2, *gmm.params()).reshape(lead)
+
+    def sample(self, shape: Size = ()) -> Tensor:
+        gmm = self._call.gmm
+        D = gmm.features
+        lead = Size(shape) + self._batch
+        params = gmm.params()
+        device = params[0].device
+        n = prod(lead)
+        with torch.no_grad():
+            u = torch.rand(n, device=device)
+            z = torch.randn(n, D, device=device)
+            c2, ldc = self._rows(lead)
+            x = torch.empty(n, D, device=device)
+            with torch.cuda.device(device):
+                h = gmm.handle(params)
+                table = _table(gmm, params)
+                need = E.lib().zk_gmm_workspace_bytes(h, n)
+                ws = E.Workspace.get(device, need, E.lib().zk_gmm_min_workspace_bytes(h))
+                E.check(E.lib().zk_gmm_sample(h, _ptr(c2), ldc, _ptr(table), u.data_ptr(), z.data_ptr(), D, n,
+                                              x.data_ptr(), D, ws.data_ptr(), ws.numel(), E.stream_ptr(device)))  # fmt: skip
+        return x.reshape(*lead, D)
+
+
+def _ptr(t: Tensor | None) -> int | None:
+    return None if t is None else t.data_ptr()
+
+
+def _table(gmm, params) -> Tensor | None:  # noqa: ANN001
+    """The unconditional parameter row (``phi`` flattened in unpack order); ``None`` for a conditional model."""
+    if hasattr(gmm, "hyper"):
+        return None
+    return torch.cat([p.detach().reshape(-1) for p in params]).contiguous()
+
+
+class _MixtureLogProb(torch.autograd.Function):
+    """``Mixture.log_prob`` on engine rows: forward = ``zk_gmm_log_prob``, backward = ``zk_gmm_backward``
+    (gradients of x, of the context rows and of every tensor of ``GMM.params()``)."""
+
+    @staticmethod
+    def forward(ctx, gmm, ldc, x2, c2, *params):  # noqa: ANN001
+        E.require_cuda(x2, "input")
+        B, D = x2.shape
+        device = x2.device
+        out = torch.empty(B, device=device, dtype=torch.float32)
+        with torch.cuda.device(device):
+            h = gmm.handle(params)
+            table = _table(gmm, params)
+            need = E.lib().zk_gmm_workspace_bytes(h, B)
+            ws = E.Workspace.get(device, need, E.lib().zk_gmm_min_workspace_bytes(h))
+            E.check(E.lib().zk_gmm_log_prob(h, x2.data_ptr(), D, _ptr(c2), ldc, _ptr(table), B, out.data_ptr(),
+                                            ws.data_ptr(), ws.numel(), E.stream_ptr(device)))  # fmt: skip
+        ctx.gmm, ctx.ldc, ctx.has_c = gmm, ldc, c2 is not None
+        ctx.save_for_backward(x2, *(() if c2 is None else (c2,)), *params)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):  # noqa: ANN001
+        gmm, ldc = ctx.gmm, ctx.ldc
+        saved = ctx.saved_tensors
+        x2, c2 = saved[0], (saved[1] if ctx.has_c else None)
+        params = saved[2 if ctx.has_c else 1 :]
+        need = ctx.needs_input_grad
+        B, D = x2.shape
+        device = x2.device
+        g = g.contiguous()
+        gx = torch.empty_like(x2) if need[2] else None
+        gc = torch.zeros_like(c2) if c2 is not None and need[3] else None
+        grads = [torch.zeros_like(p) for p in params]
+        keep = []
+        if hasattr(gmm, "hyper"):
+            weights, biases = gmm._split(grads)
+            W = (ctypes.c_void_p * len(weights))(*[w.data_ptr() for w in weights])
+            Bv = (ctypes.c_void_p * len(biases))(*[None if b is None else b.data_ptr() for b in biases])
+            keep += [W, Bv]
+            layer_grads = E.LayerGrads(ctypes.cast(W, ctypes.POINTER(ctypes.c_void_p)), ctypes.cast(Bv, ctypes.POINTER(ctypes.c_void_p)), None, None)  # noqa: E501
+            flat = None
+        else:
+            flat = torch.zeros(gmm.total, device=device)
+            layer_grads = E.LayerGrads(None, None, flat.data_ptr(), None)
+        with torch.cuda.device(device):
+            h = gmm.handle(params)
+            table = _table(gmm, params)
+            want = E.lib().zk_gmm_backward_workspace_bytes(h, B)
+            ws = E.Workspace.get(device, want, E.lib().zk_gmm_min_workspace_bytes(h))
+            E.check(E.lib().zk_gmm_backward(h, x2.data_ptr(), D, _ptr(c2), ldc, _ptr(table), B, g.data_ptr(), _ptr(gx), D,
+                                            _ptr(gc), 0 if c2 is None else c2.shape[-1], ctypes.byref(layer_grads),
+                                            ws.data_ptr(), ws.numel(), E.stream_ptr(device)))  # fmt: skip
+        if flat is not None:
+            grads = [part.reshape(p.shape) for part, p in zip(flat.split([p.numel() for p in params]), params, strict=True)]
+        return (None, None, gx, gc, *[gr if n else None for gr, n in zip(grads, need[4:], strict=True)])

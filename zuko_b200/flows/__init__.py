@@ -5,12 +5,14 @@ from .continuous import CNF, FFJTransform
 from .coupling import NICE, GeneralCouplingTransform, RealNVP
 from .elementwise import ElementWiseTransform
 from .gaussianization import GF
+from .mixture import GMM
 from .polynomial import BPF, SOSPF
 from .spline import NCSF, NSF
 from ..lazy import Flow, UnconditionalDistribution, UnconditionalTransform
 
 __all__ = [
     "GF",
+    "GMM",
     "MAF",
     "NCSF",
     "NICE",
