@@ -63,8 +63,8 @@ constexpr uint32_t F_TILE = FM * FK * 2;  // 8 KB: one plane of a 64 x 64 tile
 constexpr uint32_t F_STAGE = 2 * F_TILE;  // hi + lo
 constexpr uint32_t F_SMEM_MAX = 232448;   // 227 KB per block on sm_90
 
-// floats per row of the output-layer staging region: the chunk's DPC * P parameters, made odd.  The region is still
-// allocated (it sizes the plan) but no longer used: output chunks are assembled in registers
+// floats per row of the former output-layer staging region: the chunk's DPC * P parameters, made odd.  The region
+// still sizes the plan; output chunks are assembled in registers, and the region holds the hidden layers' biases
 __host__ __device__ constexpr int f_srow(int dpc_p) { return dpc_p | 1; }
 
 struct FusedParams {
@@ -130,7 +130,7 @@ __global__ void __launch_bounds__(F_THREADS, 1)
 fused_layer_kernel(const __grid_constant__ FusedParams p) {
     using Cfg = LastCfg<UNI, KT>;
     constexpr int P = Cfg::P, DPC = Cfg::DPC, NL = Cfg::NL;
-    constexpr int NP = DPC * P, SROW = f_srow(NP);  // parameters of an output chunk, row stride of the unused region
+    constexpr int NP = DPC * P, SROW = f_srow(NP);  // parameters of an output chunk, row stride of the bias region
     constexpr bool WIDE = (ROWS == 128);
     using Out = outchunk::Shape<P, DPC>;
     static_assert(NP <= NL && NL <= FK && NL % 8 == 0 && Out::NCOL <= NL, "a last-layer chunk must fit its MMA width");
@@ -139,13 +139,15 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    // [W ring: n_stages x 16 KB][A: ROWS / 64 x 2 planes x KBA x 8 KB][unused: 2 x 64 x SROW fp32]
+    // [W ring: n_stages x 16 KB][A: ROWS / 64 x 2 planes x KBA x 8 KB][hidden biases: region of 2 x 64 x SROW fp32]
     // [ladj partials 4 x ROWS][barriers]
     const int NS = p.n_stages;
     uint8_t* sW = smem;
     uint8_t* sA = smem + (size_t)NS * F_STAGE;
     const uint32_t a_plane = (uint32_t)p.KBA * F_TILE;
-    float* s_part = (float*)(sA + (ROWS / FM) * 2 * (size_t)a_plane) + 2 * FM * SROW;
+    float* s_bias = (float*)(sA + (ROWS / FM) * 2 * (size_t)a_plane);  // [L - 1][H]
+    static_assert(2 * FM * SROW >= (ZK_FUSED_MAX_LINEAR - 1) * F_MAXKB * FK, "the hidden biases fit the region");
+    float* s_part = s_bias + 2 * FM * SROW;
     uint64_t* full = (uint64_t*)(s_part + 4 * ROWS);         // [F_MAX_STAGES] TMA -> consumer
     uint64_t* empty = full + F_MAX_STAGES;                   // [F_MAX_STAGES] consumer -> TMA
     const int NR = WIDE ? NS : NS / 2;                       // slots per ring (64 rows: ring g = [g NR, g NR + NR))
@@ -209,6 +211,11 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
     auto release = [&](int slot) { if (tid == 0) mbar_arrive(&empty[slot]); };
     // the threads that read and write this warpgroup's A operand
     auto sync_a = [&]() { if constexpr (WIDE) named_bar_sync(2 + cw, 128); else named_bar_sync(1, 256); };
+
+    // the hidden layers' biases, once per CTA: the epilogues read them from shared memory rather than waiting on a
+    // global load per chunk
+    for (int i = ctid; i < (L - 1) * p.H; i += 256) s_bias[i] = __ldg(p.bias[i / p.H] + i % p.H);
+    named_bar_sync(1, 256);
 
     for (int t = blockIdx.x; t < m_tiles; t += gridDim.x) {
         const int64_t rb = (int64_t)t * ROWS + (WIDE ? cw * FM : 0);  // first row of this warpgroup's A
@@ -316,7 +323,7 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
                 }
             }
             sync_a();  // every reader of this A operand is done with it: overwrite it
-            const float* bias = p.bias[l];
+            const uint32_t bias = smem_u32(s_bias + l * p.H);
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 const int ch = WIDE ? q : 2 * q + cw;
@@ -329,7 +336,7 @@ fused_layer_kernel(const __grid_constant__ FusedParams p) {
 #pragma unroll
                     for (int di = 0; di < 2; ++di) {
                         const int i = i0 + di;
-                        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + ch * FK + 8 * i + 2 * (lane & 3)));
+                        const float2 bb = lds_f32x2(bias + 4u * (uint32_t)(ch * FK + 8 * i + 2 * (lane & 3)));
 #pragma unroll
                         for (int hh = 0; hh < 2; ++hh) {
                             float v[2] = {acc[q][4 * i + 2 * hh] + bb.x, acc[q][4 * i + 2 * hh + 1] + bb.y};

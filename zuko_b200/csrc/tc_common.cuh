@@ -127,6 +127,13 @@ __device__ __forceinline__ void wgmma_kblock(float (&d)[NA], uint32_t a_hi, uint
     }
 }
 
+// two consecutive fp32 at a shared-memory address (shared window)
+__device__ __forceinline__ float2 lds_f32x2(uint32_t addr) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+    return v;
+}
+
 // four 8 x 8 b16 matrices to shared memory: lane l gives the address of row l % 8 of matrix l / 8 (16 bytes), and
 // r[m] is the pair of matrix m at row l / 4, columns 2 (l % 4), 2 (l % 4) + 1 — an 8 x 8 block of the wgmma
 // accumulator fragment after packing to bf16x2
