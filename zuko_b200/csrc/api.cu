@@ -355,6 +355,19 @@ zk_status zk_layer_destroy(zk_layer* l) {
     return ZK_OK;
 }
 
+// the step-ordered weights of an autoregressive layer's dimension-sequential inverse, from the conditioner's masks
+// and the order classes; no pack when its per-thread state does not fit (the inverse then runs the sweeps)
+static zk_status build_inverse_pack(zk_layer* l, const uint8_t* const* mask, const int64_t* order) {
+    ZK_TRY(ar_inverse_pack(l->hyper, mask, order, l->D, l->C, l->spec, l->passes, &l->inv));
+    int T = 0;
+    size_t smem = 0;
+    if (l->inv && !ar_inverse_threads(l->inv, &T, &smem)) {
+        ar_inverse_free(l->inv);
+        l->inv = nullptr;
+    }
+    return ZK_OK;
+}
+
 static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
     l->kind = d->kind; l->D = d->features; l->C = d->context; l->passes = d->passes;
     l->spec = UniSpec{d->univariate, d->bins, d->degree, d->bound, d->slope, kBernsteinEps, d->iterations};
@@ -388,16 +401,7 @@ static zk_status layer_create_impl(const zk_layer_desc* d, zk_layer* l) {
                        l->hyper->dims[l->hyper->n_linear], l->D * l->P);
             ZK_TRY(fused_layer_prepare(l->hyper, d->hyper->mask, l->spec.kind, l->spec.K, l->D, l->C));
             if (d->order) l->order.assign(d->order, d->order + l->D);
-            {
-                int T = 0;
-                size_t smem = 0;
-                ZK_TRY(ar_inverse_pack(l->hyper, d->hyper->mask, d->order, l->D, l->C, l->spec, l->passes, &l->inv));
-                if (l->inv && !ar_inverse_threads(l->inv, &T, &smem)) {  // state too large: use the sweeps
-                    ar_inverse_free(l->inv);
-                    l->inv = nullptr;
-                }
-            }
-            return ZK_OK;
+            return build_inverse_pack(l, d->hyper->mask, d->order);
         }
         case ZK_LAYER_COUPLING: {
             ZK_REQUIRE(d->hyper && d->coupling_mask, "layer_create: coupling layer needs conditioner and mask");
@@ -587,6 +591,49 @@ bool layer_can_fuse_base(const zk_layer* l) {
     return l->kind == ZK_LAYER_AUTOREGRESSIVE || l->kind == ZK_LAYER_ELEMENTWISE;
 }
 
+// One pass of a conditioned layer (autoregressive, coupling, element-wise): the conditioner reads `xc` and the
+// context and gives phi, then one bijector pass maps `xb` to `out` in the direction a.inverse (`a` carries the
+// spec, the batch and the ladj / log_prob outputs).  The two inputs differ only in the autoregressive inverse
+// sweeps, whose conditioner reads the iterate.
+static zk_status conditioned_pass(const zk_layer* l, UniArgs a, const float* xc, int64_t ldxc, const float* xb,
+                                  int64_t ldxb, const float* c, int64_t ldc, float* out, int64_t ldo, void* ws,
+                                  size_t ws_bytes, cudaStream_t st) {
+    a.x = xb; a.ldx = ldxb; a.y = out; a.ldy = ldo; a.D = l->D;
+    if (!l->hyper) {  // element-wise layer with one shared (D, P) table
+        a.phi = l->phi_shared;
+        a.phi_ld = 0;
+        return launch_univariate(a, st);
+    }
+    const int64_t B = a.B;
+    const bool coupling = (l->kind == ZK_LAYER_COUPLING);
+    const bool bcast = (l->kind == ZK_LAYER_ELEMENTWISE && ldc == 0);  // broadcast context => one shared table
+    if (coupling) a.D = l->n_b;                                         // the transformed dims
+    const int64_t ldphi = (int64_t)a.D * l->P;
+    Arena ar(ws, ws_bytes);
+    float* phi = ar.take<float>((size_t)(bcast ? 1 : B) * ldphi);
+    float* xa = coupling ? ar.take<float>((size_t)B * l->n_a) : nullptr;
+    ZK_REQUIRE(ar.ok, "%s: workspace too small", a.inverse ? "layer_inverse" : "layer_forward");
+    void* mws = ar.base + ar.off;
+    const size_t mws_bytes = ar.size - ar.off;
+    switch (l->kind) {
+        case ZK_LAYER_AUTOREGRESSIVE:  // flows/autoregressive.py:207-215
+            ZK_TRY(zk_mlp_forward(l->hyper, xc, ldxc, l->D, c, ldc, l->C, B, phi, ldphi, mws, mws_bytes, st));
+            break;
+        case ZK_LAYER_COUPLING:  // forward transforms.py:1067-1072, inverse 1054-1058; flows/coupling.py:128-136
+            gather_columns_kernel<<<(unsigned)ceil_div(B * l->n_a, 256), 256, 0, st>>>(xc, ldxc, l->idx_a, l->n_a, B, xa);
+            ZK_TRY(check_launch("gather_columns_kernel"));
+            ZK_TRY(zk_mlp_forward(l->hyper, xa, l->n_a, l->n_a, c, ldc, l->C, B, phi, ldphi, mws, mws_bytes, st));
+            if (out) ZK_TRY(launch_copy_columns(xb, ldxb, l->idx_a, l->n_a, B, out, ldo, st));
+            a.dim_map = l->idx_b;
+            break;
+        default:  // element-wise, flows/gaussianization.py:86-94: phi = hyper(c)
+            ZK_TRY(zk_mlp_forward(l->hyper, c, ldc, l->C, nullptr, 0, 0, bcast ? 1 : B, phi, ldphi, mws, mws_bytes, st));
+    }
+    a.phi = phi;
+    a.phi_ld = bcast ? 0 : ldphi;
+    return launch_univariate(a, st);
+}
+
 // Forward of one layer.  When log_prob != nullptr (only for layers where
 // layer_can_fuse_base) the DiagNormal term is fused and y may be nullptr.
 zk_status layer_forward_impl(const zk_layer* l, const float* x, int64_t ldx, const float* c,
@@ -595,7 +642,6 @@ zk_status layer_forward_impl(const zk_layer* l, const float* x, int64_t ldx, con
                              void* ws, size_t ws_bytes, cudaStream_t st) {
     if (B == 0) return ZK_OK;
     ZK_REQUIRE(l->C == 0 || c != nullptr, "layer needs a context of %d features", l->C);
-    Arena ar(ws, ws_bytes);
     UniArgs a;
     a.spec = l->spec; a.B = B;
     a.ladj = ladj; a.accumulate = accumulate; a.log_prob = log_prob; a.base_loc = loc;
@@ -613,45 +659,11 @@ zk_status layer_forward_impl(const zk_layer* l, const float* x, int64_t ldx, con
                 f.base_scale = scale; f.fast_math = g_fast_math.load() != 0;
                 return launch_fused_layer(l->hyper, f, st);
             }
-            float* phi = ar.take<float>((size_t)B * l->D * l->P);
-            ZK_REQUIRE(ar.ok, "layer_forward: workspace too small");
-            ZK_TRY(zk_mlp_forward(l->hyper, x, ldx, l->D, c, ldc, l->C, B, phi, (int64_t)l->D * l->P,
-                                  ar.base + ar.off, ar.size - ar.off, st));
-            a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = (int64_t)l->D * l->P; a.D = l->D;
-            a.y = y; a.ldy = ldy;
-            return launch_univariate(a, st);
+            [[fallthrough]];
         }
-        case ZK_LAYER_COUPLING: {
-            // transforms.py:1067-1072 + flows/coupling.py:128-136
-            float* phi = ar.take<float>((size_t)B * l->n_b * l->P);
-            float* xa = ar.take<float>((size_t)B * l->n_a);
-            ZK_REQUIRE(ar.ok, "layer_forward: workspace too small");
-            gather_columns_kernel<<<(unsigned)ceil_div(B * l->n_a, 256), 256, 0, st>>>(x, ldx, l->idx_a, l->n_a, B, xa);
-            ZK_TRY(check_launch("gather_columns_kernel"));
-            ZK_TRY(zk_mlp_forward(l->hyper, xa, l->n_a, l->n_a, c, ldc, l->C, B, phi, (int64_t)l->n_b * l->P,
-                                  ar.base + ar.off, ar.size - ar.off, st));
-            if (y) ZK_TRY(launch_copy_columns(x, ldx, l->idx_a, l->n_a, B, y, ldy, st));
-            a.x = x; a.ldx = ldx; a.phi = phi; a.phi_ld = (int64_t)l->n_b * l->P; a.D = l->n_b;
-            a.y = y; a.ldy = ldy; a.dim_map = l->idx_b;
-            return launch_univariate(a, st);
-        }
-        case ZK_LAYER_ELEMENTWISE: {
-            // flows/gaussianization.py:86-94
-            a.x = x; a.ldx = ldx; a.D = l->D; a.y = y; a.ldy = ldy;
-            if (l->hyper) {
-                const int64_t rows = (ldc == 0) ? 1 : B;  // broadcast context => one shared table
-                float* phi = ar.take<float>((size_t)rows * l->D * l->P);
-                ZK_REQUIRE(ar.ok, "layer_forward: workspace too small");
-                ZK_TRY(zk_mlp_forward(l->hyper, c, ldc, l->C, nullptr, 0, 0, rows, phi, (int64_t)l->D * l->P,
-                                      ar.base + ar.off, ar.size - ar.off, st));
-                a.phi = phi;
-                a.phi_ld = (ldc == 0) ? 0 : (int64_t)l->D * l->P;
-            } else {
-                a.phi = l->phi_shared;
-                a.phi_ld = 0;
-            }
-            return launch_univariate(a, st);
-        }
+        case ZK_LAYER_COUPLING:
+        case ZK_LAYER_ELEMENTWISE:
+            return conditioned_pass(l, a, x, ldx, x, ldx, c, ldc, y, ldy, ws, ws_bytes, st);
         case ZK_LAYER_SOFTCLIP:
             return launch_softclip(x, ldx, B, l->D, l->spec.bound, false, y, ldy, ladj, accumulate, st);
         case ZK_LAYER_PERMUTATION:
@@ -677,7 +689,6 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
     if (ladj_done) *ladj_done = false;
     if (B == 0) return ZK_OK;
     ZK_REQUIRE(l->C == 0 || c != nullptr, "layer needs a context of %d features", l->C);
-    Arena ar(ws, ws_bytes);
     UniArgs a;
     a.spec = l->spec; a.inverse = true; a.B = B; a.fast_math = g_fast_math.load() != 0;
     switch (l->kind) {
@@ -691,14 +702,7 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
                     ZK_CUDA(cudaStreamSynchronize(st));  // the refresh kernels ran on the caller's stream
                     ar_inverse_free(ml->inv);
                     ml->inv = nullptr;
-                    int T = 0;
-                    size_t smem = 0;
-                    ZK_TRY(ar_inverse_pack(ml->hyper, ml->hyper->mask.data(), ml->order.empty() ? nullptr : ml->order.data(), ml->D,
-                                           ml->C, ml->spec, ml->passes, &ml->inv));
-                    if (ml->inv && !ar_inverse_threads(ml->inv, &T, &smem)) {
-                        ar_inverse_free(ml->inv);
-                        ml->inv = nullptr;
-                    }
+                    ZK_TRY(build_inverse_pack(ml, ml->hyper->mask.data(), ml->order.empty() ? nullptr : ml->order.data()));
                     ml->inv_dirty = false;
                 }
             }
@@ -713,52 +717,18 @@ zk_status layer_inverse_impl(const zk_layer* l, const float* y, int64_t ldy, con
                 }
                 return launch_ar_inverse(l->inv, ia, st);
             }
-            float* phi = ar.take<float>((size_t)B * l->D * l->P);
-            ZK_REQUIRE(ar.ok, "layer_inverse: workspace too small");
             if (ldx == l->D) {
                 ZK_CUDA(cudaMemsetAsync(x, 0, (size_t)B * l->D * 4, st));
             } else {
                 ZK_CUDA(cudaMemset2DAsync(x, (size_t)ldx * 4, 0, (size_t)l->D * 4, (size_t)B, st));
             }
-            a.x = y; a.ldx = ldy; a.phi = phi; a.phi_ld = (int64_t)l->D * l->P; a.D = l->D;
-            a.y = x; a.ldy = ldx;
-            for (int p = 0; p < l->passes; ++p) {
-                ZK_TRY(zk_mlp_forward(l->hyper, x, ldx, l->D, c, ldc, l->C, B, phi, (int64_t)l->D * l->P,
-                                      ar.base + ar.off, ar.size - ar.off, st));
-                ZK_TRY(launch_univariate(a, st));
-            }
+            for (int p = 0; p < l->passes; ++p)  // the conditioner reads the iterate x, the bijector inverts y
+                ZK_TRY(conditioned_pass(l, a, x, ldx, y, ldy, c, ldc, x, ldx, ws, ws_bytes, st));
             return ZK_OK;
         }
-        case ZK_LAYER_COUPLING: {
-            // transforms.py:1054-1058
-            float* phi = ar.take<float>((size_t)B * l->n_b * l->P);
-            float* ya = ar.take<float>((size_t)B * l->n_a);
-            ZK_REQUIRE(ar.ok, "layer_inverse: workspace too small");
-            gather_columns_kernel<<<(unsigned)ceil_div(B * l->n_a, 256), 256, 0, st>>>(y, ldy, l->idx_a, l->n_a, B, ya);
-            ZK_TRY(check_launch("gather_columns_kernel"));
-            ZK_TRY(zk_mlp_forward(l->hyper, ya, l->n_a, l->n_a, c, ldc, l->C, B, phi, (int64_t)l->n_b * l->P,
-                                  ar.base + ar.off, ar.size - ar.off, st));
-            ZK_TRY(launch_copy_columns(y, ldy, l->idx_a, l->n_a, B, x, ldx, st));
-            a.x = y; a.ldx = ldy; a.phi = phi; a.phi_ld = (int64_t)l->n_b * l->P; a.D = l->n_b;
-            a.y = x; a.ldy = ldx; a.dim_map = l->idx_b;
-            return launch_univariate(a, st);
-        }
-        case ZK_LAYER_ELEMENTWISE: {
-            a.x = y; a.ldx = ldy; a.D = l->D; a.y = x; a.ldy = ldx;
-            if (l->hyper) {
-                const int64_t rows = (ldc == 0) ? 1 : B;
-                float* phi = ar.take<float>((size_t)rows * l->D * l->P);
-                ZK_REQUIRE(ar.ok, "layer_inverse: workspace too small");
-                ZK_TRY(zk_mlp_forward(l->hyper, c, ldc, l->C, nullptr, 0, 0, rows, phi, (int64_t)l->D * l->P,
-                                      ar.base + ar.off, ar.size - ar.off, st));
-                a.phi = phi;
-                a.phi_ld = (ldc == 0) ? 0 : (int64_t)l->D * l->P;
-            } else {
-                a.phi = l->phi_shared;
-                a.phi_ld = 0;
-            }
-            return launch_univariate(a, st);
-        }
+        case ZK_LAYER_COUPLING:
+        case ZK_LAYER_ELEMENTWISE:
+            return conditioned_pass(l, a, y, ldy, y, ldy, c, ldc, x, ldx, ws, ws_bytes, st);
         case ZK_LAYER_SOFTCLIP:
             return launch_softclip(y, ldy, B, l->D, l->spec.bound, true, x, ldx, nullptr, 0, st);
         case ZK_LAYER_PERMUTATION:
@@ -803,17 +773,16 @@ size_t flow_ws_for(const zk_flow_desc* f, int64_t Bc, int dir = 0) {
            + a256(reduce_scratch_bytes()) + layer_max + 1024;
 }
 
-int64_t flow_chunk_rows(const zk_flow_desc* f, int64_t B, size_t ws_bytes, int dir = 0) {
-    if (flow_ws_for(f, B, dir) <= ws_bytes) return B;
-    int64_t lo = 1, hi = B;  // largest chunk that fits (monotone in Bc)
-    if (flow_ws_for(f, 1, dir) > ws_bytes) return 0;
-    while (lo < hi) {
-        int64_t mid = lo + (hi - lo + 1) / 2;
-        if (flow_ws_for(f, mid, dir) <= ws_bytes) lo = mid; else hi = mid - 1;
-    }
-    // keep tiles aligned: round down to a multiple of 1024 rows when possible
-    if (lo >= 2048) lo = lo / 1024 * 1024;
-    return lo;
+int64_t flow_chunk_rows(const zk_flow_desc* f, int64_t B, size_t ws_bytes, int dir) {
+    return largest_fitting_rows(B, ws_bytes, [&](int64_t n) { return flow_ws_for(f, n, dir); }, 1024);
+}
+
+// base.log_prob(z) (+ ladj when given) into out
+static zk_status base_log_prob(const zk_flow_desc* f, const float* z, int64_t ldz, const float* ladj, int64_t B,
+                               float* out, cudaStream_t st) {
+    if (f->base_kind == ZK_BASE_BOX_UNIFORM)
+        return launch_box_uniform(z, ldz, f->base_loc, f->base_scale, ladj, B, f->features, out, st);
+    return launch_diag_normal(z, ldz, f->base_loc, f->base_scale, ladj, B, f->features, out, st);
 }
 
 zk_status flow_check(const zk_flow_desc* f) {
@@ -893,12 +862,7 @@ zk_status flow_forward_chunk(const zk_flow_desc* f, const float* x, int64_t ldx,
         ZK_TRY(launch_fill(ladj, B, 0.f, st));
         if (z) ZK_TRY(copy_rows(x, ldx, B, D, z, ldz, st));
     }
-    if (log_prob && !fused) {
-        if (f->base_kind == ZK_BASE_BOX_UNIFORM)
-            ZK_TRY(launch_box_uniform(cur, ldcur, f->base_loc, f->base_scale, ladj, B, D, log_prob, st));
-        else
-            ZK_TRY(launch_diag_normal(cur, ldcur, f->base_loc, f->base_scale, ladj, B, D, log_prob, st));
-    }
+    if (log_prob && !fused) ZK_TRY(base_log_prob(f, cur, ldcur, ladj, B, log_prob, st));
     return ZK_OK;
 }
 
@@ -948,10 +912,7 @@ zk_status flow_inverse_chunk(const zk_flow_desc* f, const float* z, int64_t ldz,
                 seeded = true;
             } else {
                 if (!seeded) {  // base log-density of z = the first inverted layer's input
-                    if (f->base_kind == ZK_BASE_BOX_UNIFORM)
-                        ZK_TRY(launch_box_uniform(z, ldz, f->base_loc, f->base_scale, nullptr, B, D, log_prob, st));
-                    else
-                        ZK_TRY(launch_diag_normal(z, ldz, f->base_loc, f->base_scale, nullptr, B, D, log_prob, st));
+                    ZK_TRY(base_log_prob(f, z, ldz, nullptr, B, log_prob, st));
                     seeded = true;
                 }
                 // forward ladj of this layer alone at its input `dst`; its output is not needed and goes to
@@ -967,12 +928,7 @@ zk_status flow_inverse_chunk(const zk_flow_desc* f, const float* z, int64_t ldz,
     }
     if (T == 0) {
         ZK_TRY(copy_rows(z, ldz, B, D, x, ldx, st));
-        if (want) {
-            if (f->base_kind == ZK_BASE_BOX_UNIFORM)
-                ZK_TRY(launch_box_uniform(z, ldz, f->base_loc, f->base_scale, nullptr, B, D, log_prob, st));
-            else
-                ZK_TRY(launch_diag_normal(z, ldz, f->base_loc, f->base_scale, nullptr, B, D, log_prob, st));
-        }
+        if (want) ZK_TRY(base_log_prob(f, z, ldz, nullptr, B, log_prob, st));
     }
     return ZK_OK;
 }

@@ -31,8 +31,6 @@ std::atomic<int> g_tc_backward{1};
 
 }  // namespace
 
-bool tc_backward_on() { return g_tc_backward.load() != 0; }
-
 // transposed pre-masked weights for dgrad, built on first use
 zk_status mlp_ensure_backward(const zk_mlp* cm, cudaStream_t st) {
     zk_mlp* m = const_cast<zk_mlp*>(cm);
@@ -257,6 +255,49 @@ zk_status tc_mlp_backward(const zk_mlp* m, const TcBwdPlan& p, const TcBwdBufs& 
     return ZK_OK;
 }
 
+static bool backward_on_tc(const zk_mlp* m, bool allow_tc) {
+    return allow_tc && mlp_uses_tc(m) && g_tc_backward.load();
+}
+
+size_t ConditionerBackward::bytes(const zk_mlp* mlp, int64_t rows, bool allow_tc) {
+    return backward_on_tc(mlp, allow_tc) ? tc_bwd_ws(mlp, rows) : mlp_bwd_ws(mlp, rows);
+}
+
+zk_status ConditionerBackward::recompute(const zk_mlp* mlp, bool allow_tc, const float* x, int64_t ldx, const int* cols,
+                                         int nx, const float* c, int64_t ldc, int nc, int64_t rows, Arena& ar,
+                                         const char* what, cudaStream_t st) {
+    m = mlp;
+    B = rows;
+    tc = backward_on_tc(m, allow_tc);
+    ZK_TRY(mlp_ensure_backward(m, st));
+    if (tc) {
+        plan = tc_plan(m, B);
+        ZK_REQUIRE(tc_bwd_carve(m, plan, B, ar, tb), "%s: workspace too small", what);
+        ZK_TRY(launch_concat(x, ldx, cols, nx, c, ldc, nc, B, tb.a0, st));
+        ZK_TRY(tc_forward_save(m, plan, tb, B, st));
+        phi = tb.out;
+        scratch = tb.scratch;
+        return ZK_OK;
+    }
+    ZK_REQUIRE(mlp_bwd_carve(m, B, ar, mb), "%s: workspace too small", what);
+    ZK_TRY(launch_concat(x, ldx, cols, nx, c, ldc, nc, B, mb.acts[0], st));
+    ZK_TRY(mlp_forward_save(m, mb, B, st));
+    phi = mb.out;
+    scratch = mb.scratch;
+    return ZK_OK;
+}
+
+zk_status ConditionerBackward::backward(float* gphi, bool want_gin, const zk_layer_grads* grads, cudaStream_t st) {
+    if (tc) {
+        tb.out = gphi;
+        gin = tb.gin;
+        return tc_mlp_backward(m, plan, tb, B, want_gin, grads, st);
+    }
+    mb.out = gphi;
+    gin = mb.gin;
+    return mlp_backward(m, mb, B, want_gin, grads, st);
+}
+
 namespace {
 
 size_t layer_bwd_ws(const zk_layer* l, int64_t B) {
@@ -293,43 +334,23 @@ zk_status layer_backward_impl(const zk_layer* l, const float* x, int64_t ldx, co
         case ZK_LAYER_AUTOREGRESSIVE:
         case ZK_LAYER_COUPLING: {
             const bool coupling = (l->kind == ZK_LAYER_COUPLING);
-            const zk_mlp* m = l->hyper;
             const int nx = coupling ? l->n_a : l->D;
             const int nt = coupling ? l->n_b : l->D;  // transformed dims
-            ZK_TRY(mlp_ensure_backward(m, st));
-            u.phi_ld = (int64_t)nt * l->P; u.D = nt;
+            const int* cols = coupling ? l->idx_a : nullptr;
+            ConditionerBackward cb;
+            ZK_TRY(cb.recompute(l->hyper, true, x, ldx, cols, nx, c, ldc, l->C, B, ar, "layer_backward", st));
+            u.phi = cb.phi; u.phi_ld = (int64_t)nt * l->P; u.D = nt;
             u.dim_map = coupling ? l->idx_b : nullptr;
-            const bool per_row_gc = (gc != nullptr && l->C > 0 && ldc != 0);
-            if (mlp_uses_tc(m) && g_tc_backward.load()) {
-                // tensor-core path: forward recompute, dgrad and wgrad on linear_tc_kernel
-                const TcBwdPlan plan = tc_plan(m, B);
-                TcBwdBufs tb;
-                ZK_REQUIRE(tc_bwd_carve(m, plan, B, ar, tb), "layer_backward: workspace too small");
-                ZK_TRY(launch_concat(x, ldx, coupling ? l->idx_a : nullptr, nx, c, ldc, l->C, B, tb.a0, st));
-                ZK_TRY(tc_forward_save(m, plan, tb, B, st));
-                u.phi = tb.out; u.gphi = direct_only ? nullptr : tb.out;
-                ZK_TRY(launch_univariate_backward(u, st));
-                if (direct_only) return ZK_OK;
-                ZK_TRY(tc_mlp_backward(m, plan, tb, B, true, grads, st));
-                ZK_TRY(launch_input_grad(tb.gin, nx, l->C, coupling ? l->idx_a : nullptr, B, gx, ldgx,
-                                         coupling ? gy : nullptr, ldgy, per_row_gc ? gc : nullptr, ldgc, st));
-                if (gc != nullptr && l->C > 0 && ldc == 0)
-                    ZK_TRY(launch_colsum_add(tb.gin + nx, m->dims[0], B, l->C, gc, tb.scratch, st));
-                return ZK_OK;
-            }
-            MlpBwdBufs b;
-            ZK_REQUIRE(mlp_bwd_carve(m, B, ar, b), "layer_backward: workspace too small");
-            ZK_TRY(launch_concat(x, ldx, coupling ? l->idx_a : nullptr, nx, c, ldc, l->C, B, b.acts[0], st));
-            ZK_TRY(mlp_forward_save(m, b, B, st));
-            u.phi = b.out; u.gphi = direct_only ? nullptr : b.out;
+            u.gphi = direct_only ? nullptr : cb.phi;
             ZK_TRY(launch_univariate_backward(u, st));  // gx[:, transformed] = direct term
             if (direct_only) return ZK_OK;
-            ZK_TRY(mlp_backward(m, b, B, true, grads, st));
+            ZK_TRY(cb.backward(cb.phi, true, grads, st));
             // coupling: gx[:, idx_a] = gy[:, idx_a] + gin[:, :n_a] (y_a = x_a, transforms.py:1069)
-            ZK_TRY(launch_input_grad(b.gin, nx, l->C, coupling ? l->idx_a : nullptr, B, gx, ldgx,
-                                     coupling ? gy : nullptr, ldgy, per_row_gc ? gc : nullptr, ldgc, st));
+            const bool per_row_gc = (gc != nullptr && l->C > 0 && ldc != 0);
+            ZK_TRY(launch_input_grad(cb.gin, nx, l->C, cols, B, gx, ldgx, coupling ? gy : nullptr, ldgy,
+                                     per_row_gc ? gc : nullptr, ldgc, st));
             if (gc != nullptr && l->C > 0 && ldc == 0)  // broadcast context: one summed row
-                ZK_TRY(launch_colsum_add(b.gin + nx, m->dims[0], B, l->C, gc, b.scratch, st));
+                ZK_TRY(launch_colsum_add(cb.gin + nx, l->hyper->dims[0], B, l->C, gc, cb.scratch, st));
             return ZK_OK;
         }
         case ZK_LAYER_ELEMENTWISE: {
@@ -345,34 +366,27 @@ zk_status layer_backward_impl(const zk_layer* l, const float* x, int64_t ldx, co
                 if (grads && grads->grad_phi) ZK_TRY(launch_colsum_add(rows, DP, B, DP, grads->grad_phi, scr, st));
                 return ZK_OK;
             }
-            const zk_mlp* m = l->hyper;
-            ZK_TRY(mlp_ensure_backward(m, st));
             const int64_t rows = (ldc == 0) ? 1 : B;  // gaussianization.py:89-92: phi = hyper(c)
-            MlpBwdBufs b;
-            ZK_REQUIRE(mlp_bwd_carve(m, rows, ar, b), "layer_backward: workspace too small");
-            float* grows = nullptr;
-            void* scr = nullptr;
+            // fp32 conditioner: the tensor-core path would change these gradients and the workspace figure
+            ConditionerBackward cb;
+            ZK_TRY(cb.recompute(l->hyper, false, nullptr, 0, nullptr, 0, c, ldc, l->C, rows, ar, "layer_backward", st));
+            u.phi = cb.phi;
             if (rows == 1) {
-                grows = ar.take<float>((size_t)B * DP);
-                scr = ar.take<char>(colsum_scratch_bytes(DP));
+                float* grows = ar.take<float>((size_t)B * DP);
+                void* scr = ar.take<char>(colsum_scratch_bytes(DP));
                 ZK_REQUIRE(ar.ok, "layer_backward: workspace too small");
-            }
-            ZK_TRY(launch_concat(nullptr, 0, nullptr, 0, c, ldc, l->C, rows, b.acts[0], st));
-            ZK_TRY(mlp_forward_save(m, b, rows, st));
-            u.phi = b.out;
-            if (rows == 1) {
                 u.phi_ld = 0; u.gphi = grows;
                 ZK_TRY(launch_univariate_backward(u, st));
-                ZK_CUDA(cudaMemsetAsync(b.out, 0, (size_t)DP * 4, st));
-                ZK_TRY(launch_colsum_add(grows, DP, B, DP, b.out, scr, st));
+                ZK_CUDA(cudaMemsetAsync(cb.phi, 0, (size_t)DP * 4, st));
+                ZK_TRY(launch_colsum_add(grows, DP, B, DP, cb.phi, scr, st));
             } else {
-                u.phi_ld = DP; u.gphi = b.out;
+                u.phi_ld = DP; u.gphi = cb.phi;
                 ZK_TRY(launch_univariate_backward(u, st));
             }
-            ZK_TRY(mlp_backward(m, b, rows, gc != nullptr, grads, st));
+            ZK_TRY(cb.backward(cb.phi, gc != nullptr, grads, st));
             if (gc) {
-                if (rows == 1) ZK_TRY(launch_add(gc, b.gin, l->C, st));
-                else ZK_TRY(launch_input_grad(b.gin, 0, l->C, nullptr, B, nullptr, 0, nullptr, 0, gc, ldgc, st));
+                if (rows == 1) ZK_TRY(launch_add(gc, cb.gin, l->C, st));
+                else ZK_TRY(launch_input_grad(cb.gin, 0, l->C, nullptr, B, nullptr, 0, nullptr, 0, gc, ldgc, st));
             }
             return ZK_OK;
         }
@@ -401,20 +415,6 @@ size_t flow_bwd_ws_for(const zk_flow_desc* f, int64_t Bc) {
     return (size_t)(f->n_layers + 2) * a256((size_t)Bc * D * 4)  // z_1..z_T + two gradient buffers
            + 2 * a256((size_t)Bc * 4)                            // gl, ladj scratch
            + layer_max + 1024;
-}
-
-int64_t flow_bwd_chunk_rows(const zk_flow_desc* f, int64_t B, size_t ws_bytes) {
-    if (flow_bwd_ws_for(f, B) <= ws_bytes) return B;
-    if (flow_bwd_ws_for(f, 1) > ws_bytes) return 0;
-    int64_t lo = 1, hi = B;
-    while (lo < hi) {
-        const int64_t mid = lo + (hi - lo + 1) / 2;
-        if (flow_bwd_ws_for(f, mid) <= ws_bytes) lo = mid; else hi = mid - 1;
-    }
-    // keep tiles aligned when that still fits (the batch-slice plan of the tensor-core wgrad makes the
-    // requirement only approximately monotone in the row count, so the rounded value is re-checked)
-    if (lo >= 2048 && flow_bwd_ws_for(f, lo / 1024 * 1024) <= ws_bytes) lo = lo / 1024 * 1024;
-    return lo;
 }
 
 zk_status flow_backward_chunk(const zk_flow_desc* f, const float* x, int64_t ldx, const float* c,
@@ -512,18 +512,6 @@ zk_status layer_inverse_backward_impl(const zk_layer* l, const float* x, int64_t
 
 size_t flow_invbwd_ws_for(const zk_flow_desc* f, int64_t Bc) {
     return flow_bwd_ws_for(f, Bc) + (size_t)(f->n_layers + 9) * a256((size_t)Bc * f->features * 4) + a256((size_t)Bc * 4);
-}
-
-int64_t flow_invbwd_chunk_rows(const zk_flow_desc* f, int64_t B, size_t ws_bytes) {
-    if (flow_invbwd_ws_for(f, B) <= ws_bytes) return B;
-    if (flow_invbwd_ws_for(f, 1) > ws_bytes) return 0;
-    int64_t lo = 1, hi = B;
-    while (lo < hi) {
-        const int64_t mid = lo + (hi - lo + 1) / 2;
-        if (flow_invbwd_ws_for(f, mid) <= ws_bytes) lo = mid; else hi = mid - 1;
-    }
-    if (lo >= 2048 && flow_invbwd_ws_for(f, lo / 1024 * 1024) <= ws_bytes) lo = lo / 1024 * 1024;
-    return lo;
 }
 
 zk_status flow_inverse_backward_chunk(const zk_flow_desc* f, const float* x, int64_t ldx, const float* c, int64_t ldc,
@@ -737,7 +725,8 @@ zk_status zk_flow_backward(const zk_flow_desc* f, const float* x, int64_t ldx, c
     if (C == 0) grad_c = nullptr;
     if (grad_c && ldc == 0) ZK_CUDA(cudaMemsetAsync(grad_c, 0, (size_t)C * 4, st));
     if (B == 0) return ZK_OK;
-    const int64_t Bc = flow_bwd_chunk_rows(f, B, ws_bytes);
+    // the batch-slice plan of the tensor-core wgrad makes the need only approximately monotone in the row count
+    const int64_t Bc = largest_fitting_rows(B, ws_bytes, [&](int64_t n) { return flow_bwd_ws_for(f, n); }, 1024);
     ZK_REQUIRE(Bc > 0, "flow_backward: workspace too small (%zu < %zu)", ws_bytes, zk_flow_backward_min_workspace_bytes(f));
     for (int64_t i0 = 0; i0 < B; i0 += Bc) {
         const int64_t n = std::min(Bc, B - i0);
@@ -779,7 +768,7 @@ zk_status zk_flow_inverse_backward(const zk_flow_desc* f, const float* x, int64_
     if (C == 0) grad_c = nullptr;
     if (grad_c && ldc == 0) ZK_CUDA(cudaMemsetAsync(grad_c, 0, (size_t)C * 4, st));
     if (B == 0) return ZK_OK;
-    const int64_t Bc = flow_invbwd_chunk_rows(f, B, ws_bytes);
+    const int64_t Bc = largest_fitting_rows(B, ws_bytes, [&](int64_t n) { return flow_invbwd_ws_for(f, n); }, 1024);
     ZK_REQUIRE(Bc > 0, "flow_inverse_backward: workspace too small (%zu < %zu)", ws_bytes, zk_flow_inverse_backward_min_workspace_bytes(f));
     for (int64_t i0 = 0; i0 < B; i0 += Bc) {
         const int64_t n = std::min(Bc, B - i0);

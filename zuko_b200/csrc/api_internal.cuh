@@ -42,6 +42,22 @@ inline zk_status dev_copy_from_host(const T* host, size_t n, T** out) {
     return ZK_OK;
 }
 
+// Largest row count n <= B whose workspace need(n) fits in ws_bytes; 0 when one row does not fit (or B <= 0).
+// need is monotone in n up to small bumps: with granule > 1, a count of at least two granules is rounded down
+// to a whole number of granules (aligned tiles) when the rounded count still fits.
+template <class Need>
+int64_t largest_fitting_rows(int64_t B, size_t ws_bytes, Need need, int64_t granule) {
+    if (B <= 0) return 0;
+    if (need(B) <= ws_bytes) return B;
+    if (need(1) > ws_bytes) return 0;
+    int64_t lo = 1, hi = B;
+    while (lo < hi) {
+        const int64_t mid = lo + (hi - lo + 1) / 2;
+        if (need(mid) <= ws_bytes) lo = mid; else hi = mid - 1;
+    }
+    if (granule > 1 && lo >= 2 * granule && need(lo / granule * granule) <= ws_bytes) lo = lo / granule * granule;
+    return lo;
+}
 
 }  // namespace zk
 
@@ -111,25 +127,31 @@ struct TcBwdBufs {
     void* scratch = nullptr;
 };
 
-bool tc_backward_on();  // zk_set_tc_backward
-// transposed pre-masked weights for dgrad, built on first use
-zk_status mlp_ensure_backward(const zk_mlp* cm, cudaStream_t st);
-size_t mlp_bwd_scratch(const zk_mlp* m);
-size_t mlp_bwd_ws(const zk_mlp* m, int64_t B);
-bool mlp_bwd_carve(const zk_mlp* m, int64_t B, zk::Arena& ar, MlpBwdBufs& b);
-// forward with every activation kept (fp32 CUDA-core path); acts[0] must be filled
-zk_status mlp_forward_save(const zk_mlp* m, const MlpBwdBufs& b, int64_t B, cudaStream_t st);
-// b.out holds dL/d(out) on entry; on exit b.gin = dL/d(input) when want_gin
-zk_status mlp_backward(const zk_mlp* m, const MlpBwdBufs& b, int64_t B, bool want_gin,
-                       const zk_layer_grads* grads, cudaStream_t st);
-TcBwdPlan tc_plan(const zk_mlp* m, int64_t B);
-bool mlp_uses_tc(const zk_mlp* m);
-size_t tc_bwd_ws(const zk_mlp* m, int64_t B);
-bool tc_bwd_carve(const zk_mlp* m, const TcBwdPlan& p, int64_t B, zk::Arena& ar, TcBwdBufs& b);
-// b.a0 = the conditioner input must be filled; leaves the output in b.out and every layer input in b.P
-zk_status tc_forward_save(const zk_mlp* m, const TcBwdPlan& p, const TcBwdBufs& b, int64_t B, cudaStream_t st);
-// b.out holds dL/d(out) (fp32); on exit b.gin = dL/d(input) when want_gin
-zk_status tc_mlp_backward(const zk_mlp* m, const TcBwdPlan& p, const TcBwdBufs& b, int64_t B, bool want_gin,
-                          const zk_layer_grads* grads, cudaStream_t st);
+// One conditioner backward over `rows` input rows.  recompute() carves its buffers from `ar`, writes the input
+// cat(x[:, cols] (x[:, :nx] when cols is null), c) and reruns the conditioner keeping every activation: its output
+// is `phi`.  The caller turns phi into dL/dphi (in place or in its own buffer), then backward() accumulates the
+// weight / bias gradients into `grads` and, with want_gin, leaves dL/d(input) (B, nx + nc) in `gin`; `scratch`
+// (>= colsum_scratch_bytes(nx + nc)) is free for the caller's scatter of gin.  The tensor cores run it when the
+// handle is packed for them, allow_tc is set and zk_set_tc_backward is on; otherwise the fp32 kernels do.
+struct ConditionerBackward {
+    float* phi = nullptr;
+    const float* gin = nullptr;
+    void* scratch = nullptr;
+
+    zk_status recompute(const zk_mlp* mlp, bool allow_tc, const float* x, int64_t ldx, const int* cols, int nx,
+                        const float* c, int64_t ldc, int nc, int64_t rows, zk::Arena& ar, const char* what,
+                        cudaStream_t st);
+    zk_status backward(float* gphi, bool want_gin, const zk_layer_grads* grads, cudaStream_t st);
+    // workspace of recompute() + backward() over `rows` rows, on the path they would take now
+    static size_t bytes(const zk_mlp* mlp, int64_t rows, bool allow_tc);
+
+    // kept by recompute() for backward()
+    const zk_mlp* m = nullptr;
+    int64_t B = 0;
+    bool tc = false;
+    TcBwdPlan plan;
+    TcBwdBufs tb;
+    MlpBwdBufs mb;
+};
 
 }  // namespace zkapi

@@ -132,8 +132,6 @@ GmmArgs base_args(const zk_gmm* g) {
     return a;
 }
 
-bool tc_bwd(const zk_gmm* g) { return g->hyper && mlp_uses_tc(g->hyper) && tc_backward_on(); }
-
 size_t row_bytes(const zk_gmm* g, int64_t n) { return a256((size_t)n * g->lay.total * 4); }
 
 // workspace of one call over n rows: `bcast` = one phi row for every sample (broadcast context or the
@@ -143,22 +141,15 @@ size_t ws_for(const zk_gmm* g, int64_t n, bool bwd, bool bcast) {
     const size_t colsum = a256(colsum_scratch_bytes(g->lay.total));
     if (!m) return bwd ? row_bytes(g, n) + colsum : 0;
     if (bcast)
-        return bwd ? mlp_bwd_ws(m, 1) + row_bytes(g, 1) + colsum + row_bytes(g, n)
+        return bwd ? ConditionerBackward::bytes(m, 1, false) + row_bytes(g, 1) + colsum + row_bytes(g, n)
                    : a256(zk_mlp_workspace_bytes(m, 1)) + row_bytes(g, 1);
     if (!bwd) return a256(zk_mlp_workspace_bytes(m, n)) + row_bytes(g, n);
-    return (tc_bwd(g) ? tc_bwd_ws(m, n) : mlp_bwd_ws(m, n)) + row_bytes(g, n);
+    return ConditionerBackward::bytes(m, n, true) + row_bytes(g, n);
 }
 
+// chunks are not rounded to aligned row counts: that would reorder the sums of the weight gradients
 int64_t chunk_rows(const zk_gmm* g, int64_t B, bool bwd, bool bcast, size_t bytes) {
-    if (B <= 0) return 0;
-    if (ws_for(g, B, bwd, bcast) <= bytes) return B;
-    if (ws_for(g, 1, bwd, bcast) > bytes) return 0;
-    int64_t lo = 1, hi = B;
-    while (lo < hi) {
-        const int64_t mid = lo + (hi - lo + 1) / 2;
-        if (ws_for(g, mid, bwd, bcast) <= bytes) lo = mid; else hi = mid - 1;
-    }
-    return lo;
+    return largest_fitting_rows(B, bytes, [&](int64_t n) { return ws_for(g, n, bwd, bcast); }, 1);
 }
 
 zk_status check_call(const zk_gmm* g, const float* c, const float* phi, int64_t B, const char* what) {
@@ -207,36 +198,16 @@ zk_status forward_chunks(const zk_gmm* g, const float* c, int64_t ldc, const flo
 zk_status backward_rows(const zk_gmm* g, const float* x, int64_t ldx, const float* c, int64_t ldc, int64_t n,
                         const float* glp, float* gx, int64_t ldgx, float* gc, int64_t ldgc,
                         const zk_layer_grads* grads, void* ws, size_t ws_bytes, cudaStream_t st) {
-    const zk_mlp* m = g->hyper;
     Arena ar(ws, ws_bytes);
+    ConditionerBackward cb;
+    ZK_TRY(cb.recompute(g->hyper, true, nullptr, 0, nullptr, 0, c, ldc, g->C, n, ar, "gmm_backward", st));
     GmmArgs a = base_args(g);
-    a.B = n; a.x = x; a.ldx = ldx; a.ldphi = g->lay.total; a.glp = glp; a.gx = gx; a.ldgx = ldgx;
-    if (tc_bwd(g)) {
-        const TcBwdPlan plan = tc_plan(m, n);
-        TcBwdBufs tb;
-        const bool carved = tc_bwd_carve(m, plan, n, ar, tb);
-        a.gphi = ar.take<float>((size_t)n * g->lay.total);
-        ZK_REQUIRE(carved && ar.ok, "gmm_backward: workspace too small");
-        ZK_TRY(launch_concat(nullptr, 0, nullptr, 0, c, ldc, g->C, n, tb.a0, st));
-        ZK_TRY(tc_forward_save(m, plan, tb, n, st));
-        a.phi = tb.out;
-        ZK_TRY(launch_gmm(kGmmBackward, a, st));
-        tb.out = a.gphi;
-        ZK_TRY(tc_mlp_backward(m, plan, tb, n, gc != nullptr, grads, st));
-        if (gc) ZK_TRY(launch_input_grad(tb.gin, 0, g->C, nullptr, n, nullptr, 0, nullptr, 0, gc, ldgc, st));
-        return ZK_OK;
-    }
-    MlpBwdBufs b;
-    const bool carved = mlp_bwd_carve(m, n, ar, b);
+    a.B = n; a.x = x; a.ldx = ldx; a.phi = cb.phi; a.ldphi = g->lay.total; a.glp = glp; a.gx = gx; a.ldgx = ldgx;
     a.gphi = ar.take<float>((size_t)n * g->lay.total);
-    ZK_REQUIRE(carved && ar.ok, "gmm_backward: workspace too small");
-    ZK_TRY(launch_concat(nullptr, 0, nullptr, 0, c, ldc, g->C, n, b.acts[0], st));
-    ZK_TRY(mlp_forward_save(m, b, n, st));
-    a.phi = b.out;
+    ZK_REQUIRE(ar.ok, "gmm_backward: workspace too small");
     ZK_TRY(launch_gmm(kGmmBackward, a, st));
-    b.out = a.gphi;
-    ZK_TRY(mlp_backward(m, b, n, gc != nullptr, grads, st));
-    if (gc) ZK_TRY(launch_input_grad(b.gin, 0, g->C, nullptr, n, nullptr, 0, nullptr, 0, gc, ldgc, st));
+    ZK_TRY(cb.backward(a.gphi, gc != nullptr, grads, st));
+    if (gc) ZK_TRY(launch_input_grad(cb.gin, 0, g->C, nullptr, n, nullptr, 0, nullptr, 0, gc, ldgc, st));
     return ZK_OK;
 }
 
@@ -360,7 +331,6 @@ zk_status zk_gmm_backward(const zk_gmm* g, const float* x, int64_t ldx, const fl
     const bool bcast = (g->hyper == nullptr || ldc == 0);
     const int64_t rows = chunk_rows(g, B, true, bcast, ws_bytes);
     ZK_REQUIRE(rows > 0, "gmm_backward: workspace too small (%zu < %zu)", ws_bytes, ws_for(g, 1, true, bcast));
-    if (g->hyper) ZK_TRY(mlp_ensure_backward(g->hyper, st));
     if (!bcast) {
         for (int64_t r0 = 0; r0 < B; r0 += rows) {
             const int64_t n = std::min(rows, B - r0);
@@ -371,16 +341,14 @@ zk_status zk_gmm_backward(const zk_gmm* g, const float* x, int64_t ldx, const fl
     }
     // one phi row for every sample: per-sample gradient rows, summed over the batch in a fixed order
     Arena ar(ws, ws_bytes);
-    MlpBwdBufs b;
+    ConditionerBackward cb;
     const float* row = phi;
     float* gsum = grads ? grads->grad_phi : nullptr;
-    if (g->hyper) {
-        mlp_bwd_carve(g->hyper, 1, ar, b);
+    if (g->hyper) {  // fp32 conditioner over its one row
+        ZK_TRY(cb.recompute(g->hyper, false, nullptr, 0, nullptr, 0, c, 0, g->C, 1, ar, "gmm_backward", st));
+        row = cb.phi;
         gsum = ar.take<float>(P);
         ZK_REQUIRE(ar.ok, "gmm_backward: workspace too small");
-        ZK_TRY(launch_concat(nullptr, 0, nullptr, 0, c, 0, g->C, 1, b.acts[0], st));
-        ZK_TRY(mlp_forward_save(g->hyper, b, 1, st));
-        row = b.out;
         ZK_CUDA(cudaMemsetAsync(gsum, 0, (size_t)P * 4, st));
     }
     void* scr = ar.take<char>(colsum_scratch_bytes(P));
@@ -395,9 +363,8 @@ zk_status zk_gmm_backward(const zk_gmm* g, const float* x, int64_t ldx, const fl
         if (gsum) ZK_TRY(launch_colsum_add(grows, P, a.B, P, gsum, scr, st));
     }
     if (g->hyper) {
-        b.out = gsum;
-        ZK_TRY(mlp_backward(g->hyper, b, 1, gc != nullptr, grads, st));
-        if (gc) ZK_TRY(launch_add(gc, b.gin, g->C, st));
+        ZK_TRY(cb.backward(gsum, gc != nullptr, grads, st));
+        if (gc) ZK_TRY(launch_add(gc, cb.gin, g->C, st));
     }
     return ZK_OK;
 }
