@@ -32,6 +32,8 @@ void gmm_sample_rows(const float* phi, int64_t ldphi, const float* u, const floa
     for (int64_t b = 0; b < B; ++b) zk::gmm::row_sample(phi + b * ldphi, l, eps, u[b], z + b * D, x + b * D);
 }
 
+int gmm_select_component(const float* logits, int K, float u) { return zk::gmm::select_component(logits, K, u); }
+
 int gmm_params_per_row(int D, int K, int cov, int tied) { return zk::gmm::make_layout(D, K, cov, tied).total; }
 
 }  // extern "C"

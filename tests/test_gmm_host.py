@@ -127,6 +127,52 @@ def test_row_sample_against_restatement(harness, name):
     np.testing.assert_allclose(x[ok], ref[ok], rtol=1e-5, atol=1e-5)
 
 
+def selection_uniforms(logits: np.ndarray) -> np.ndarray:
+    """u at 0, 2^-24, 1/2, the fp32 running sums of softmax(logits) and 1 - j 2^-24 for j = 1..64: the values
+    where the running sum's rounding decides the component (those below 1: u is drawn from [0, 1))."""
+    p = np.exp(logits.astype(np.float64) - logits.max())
+    p32 = (p / p.sum()).astype(np.float32)
+    sums = np.cumsum(p32, dtype=np.float32)[:-1]
+    top = 1.0 - np.arange(1, 65) * 2.0**-24
+    u = np.concatenate([[0.0, 2.0**-24, 0.5], sums, top]).astype(np.float32)
+    return u[u < 1]
+
+
+def check_selection(logits: np.ndarray, u: np.ndarray, k: np.ndarray, what: str, floor: float = 1e-30) -> None:
+    """Each draw k has an fp64 weight of at least `floor` and u lies in its fp64 CDF interval, up to the rounding of
+    the fp32 running sum (K 2^-23).  At u = 0 the inverse CDF takes the first component, whatever its weight."""
+    K = logits.size
+    p = np.exp(logits.astype(np.float64) - logits.max())
+    p /= p.sum()
+    hi = np.cumsum(p)
+    lo = hi - p
+    tol = K * 2.0**-23
+    ok = (lo[k] - tol <= u) & (u < hi[k] + tol) & ((p[k] >= floor) | ((u == 0) & (k == 0)))
+    assert ok.all(), f"{what}: u {u[~ok].tolist()} drew {k[~ok].tolist()} (weights {p[k[~ok]].tolist()})"
+
+
+@pytest.mark.parametrize("K", range(2, 33))
+def test_select_component_never_draws_a_zero_weight(harness, K):
+    """K - 1 equal logits and one at -200 or -1e4 (fp32 weight 0: exp(-200) is 1e-87) last, first or in the
+    middle, through select_component and row_sample (D = 1, means 10 k, z = 0, so x names the component).
+    Rounding leaves the fp32 running sum of the first K - 1 weights below u = 1 - 2^-24 for several K (6, 12,
+    16, 24 with glibc's expf); the last component must then not be drawn when its weight is zero."""
+    harness.gmm_select_component.restype = ctypes.c_int
+    for dead in (-200.0, -1e4):
+        for at in sorted({K - 1, 0, K // 2}):
+            logits = np.zeros(K, np.float32)
+            logits[at] = dead
+            u = selection_uniforms(logits)
+            k = np.array([harness.gmm_select_component(_ptr(logits), K, ctypes.c_float(v)) for v in u])
+            check_selection(logits, u, k, f"K={K} dead={dead} at {at}")
+            phi = np.concatenate([logits, 10.0 * np.arange(K), np.zeros(K)]).astype(np.float32)  # diagonal, untied
+            z = np.zeros((u.size, 1), np.float32)
+            x = np.empty((u.size, 1), np.float32)
+            harness.gmm_sample_rows(_ptr(phi), ctypes.c_int64(0), _ptr(u), _ptr(z), ctypes.c_int64(u.size),
+                                    *_args(1, K, "diagonal", False), _ptr(x))  # fmt: skip
+            np.testing.assert_array_equal(x[:, 0], 10.0 * k)
+
+
 @pytest.mark.parametrize("name", list(GMM_CASES))
 def test_constructor_and_state_dict_match_reference(name):
     G = load(f"gmm_{name}")

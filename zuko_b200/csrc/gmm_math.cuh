@@ -16,8 +16,8 @@
 //     dL_k = r_k (w_k v_k^T - diag(1 / L_k,ii)) on the lower triangle,   ddiag_i = dL_ii exp(diag_i)
 // (spherical: ddiag sums dL_ii over i; tied: the covariance gradients sum over k).
 // Sampling from a uniform u and a standard normal z: the component is the first k whose fixed-order
-// running sum of softmax(logits) exceeds u (the last one when rounding leaves u above the total), and
-// x = mu_k + L_k z.
+// running sum of softmax(logits) exceeds u (when rounding leaves u at or above the sum of the first K - 1,
+// the last component whose fp32 weight is positive: a zero weight is never drawn), and x = mu_k + L_k z.
 //
 // Per-row vectors (v, w, t) live behind a stride so the kernels can keep them in shared memory, one
 // column per thread.
@@ -169,15 +169,19 @@ ZK_GMM_HD float row_backward(const float* x, const float* phi, const Layout& l, 
     return out;
 }
 
-// the component u selects
+// the component u selects; never one whose fp32 weight is zero (for u >= 0 the running sum only passes
+// u at a positive weight, and the fallback is the last positive weight, not component K - 1)
 ZK_GMM_HD int select_component(const float* logits, int K, float u) {
     const float zl = lse(logits, 1, K);
     float c = 0.f;
-    for (int k = 0; k < K - 1; ++k) {
-        c += expf(logits[k] - zl);
-        if (u < c) return k;
+    int last = 0;
+    for (int k = 0; k < K; ++k) {
+        const float p = expf(logits[k] - zl);
+        if (p > 0.f) last = k;
+        c += p;
+        if (k < K - 1 && u < c) return k;
     }
-    return K - 1;
+    return last;
 }
 
 // x = mu_k + L_k z for the component u selects
