@@ -762,9 +762,11 @@ size_t flow_ws_for(const zk_flow_desc* f, int64_t Bc, int dir = 0) {
     const int D = f->features;
     size_t layer_max = 0;
     for (int i = 0; i < f->n_layers; ++i) {
-        size_t need = layer_ws_dir(f->layers[i], Bc, dir);
+        // an inverted member runs its layer's inverse in the forward direction and its forward in the inverse one
+        const int run = (dir != 0 && f->inverted && f->inverted[i]) ? 3 - dir : dir;
+        size_t need = layer_ws_dir(f->layers[i], Bc, run);
         // inverse + log_prob: a layer whose inverse kernel cannot emit its ladj runs its forward as well
-        if (dir == 2 && need != 0) need = std::max(need, layer_ws_dir(f->layers[i], Bc, 1));
+        if (run == 2 && need != 0) need = std::max(need, layer_ws_dir(f->layers[i], Bc, 1));
         layer_max = std::max(layer_max, need);
     }
     return 2 * a256((size_t)Bc * D * 4)      // ping-pong activations
@@ -800,6 +802,16 @@ zk_status flow_check(const zk_flow_desc* f) {
         if (f->inverted && f->inverted[i])
             ZK_REQUIRE(zk_layer_sequential_inverse(l), "flow: member %d is inverted but its layer has no dimension-sequential inverse", i);
     }
+    return ZK_OK;
+}
+
+// The forward direction runs an inverted member's dimension-sequential inverse, which zk_set_fused_layers(0) turns
+// off.  Refused here, before the earlier members write into the caller's outputs.
+static zk_status inverted_members_run_forward(const zk_flow_desc* f) {
+    for (int i = 0; f->inverted && i < f->n_layers; ++i)
+        if (f->inverted[i] && !g_fused.load())
+            return fail(ZK_EUNSUPPORTED, "flow: member %d is inverted; its dimension-sequential inverse does not run "
+                        "with zk_set_fused_layers(0)", i);
     return ZK_OK;
 }
 
@@ -890,8 +902,7 @@ zk_status flow_inverse_chunk(const zk_flow_desc* f, const float* z, int64_t ldz,
         float* dst = last ? x : buf[i & 1];
         const int64_t ldd = last ? ldx : D;
         if (f->inverted && f->inverted[i]) {
-            // inverse of a LazyInverse member = the layer's forward (its y; the ladj is not needed without log_prob)
-            ZK_REQUIRE(!want, "flow_inverse: log_prob of a flow with inverted members is not fused (use log_prob(x) of the result)");
+            // inverse of a LazyInverse member = the layer's forward (its y; without log_prob, zk_flow_inverse checks)
             ZK_TRY(layer_forward_impl(l, cur, ldcur, l->C ? c : nullptr, ldc, B, dst, ldd, nullptr, 0, nullptr, nullptr, nullptr,
                                       lws, lws_bytes, st));
             cur = dst;
@@ -969,6 +980,7 @@ zk_status zk_flow_forward(const zk_flow_desc* f, const float* x, int64_t ldx, co
                           int64_t ldc, int64_t B, float* z, int64_t ldz, float* ladj, void* ws,
                           size_t ws_bytes, zk_stream stream) {
     ZK_TRY(flow_check(f));
+    ZK_TRY(inverted_members_run_forward(f));
     ZK_REQUIRE(x && z && ladj, "flow_forward: null argument");
     ZK_REQUIRE(x != z, "flow_forward: z must not alias x");
     ZK_REQUIRE(B >= 0 && ldx >= f->features && ldz >= f->features, "flow_forward: bad shape");
@@ -988,6 +1000,7 @@ zk_status zk_flow_log_prob(const zk_flow_desc* f, const float* x, int64_t ldx, c
                            int64_t ldc, int64_t B, float* log_prob, double* sum_log_prob, void* ws,
                            size_t ws_bytes, zk_stream stream) {
     ZK_TRY(flow_check(f));
+    ZK_TRY(inverted_members_run_forward(f));
     ZK_REQUIRE(x && log_prob, "flow_log_prob: null argument");
     ZK_REQUIRE(B >= 0 && ldx >= f->features, "flow_log_prob: bad shape");
     ZK_REQUIRE(f->context == 0 || c, "flow_log_prob: flow needs a context");
@@ -1016,6 +1029,8 @@ zk_status zk_flow_inverse(const zk_flow_desc* f, const float* z, int64_t ldz, co
     ZK_REQUIRE(x != z, "flow_inverse: x must not alias z");
     ZK_REQUIRE(B >= 0 && ldx >= f->features && ldz >= f->features, "flow_inverse: bad shape");
     ZK_REQUIRE(f->context == 0 || c, "flow_inverse: flow needs a context");
+    for (int i = 0; log_prob && f->inverted && i < f->n_layers; ++i)
+        ZK_REQUIRE(!f->inverted[i], "flow_inverse: log_prob of a flow with inverted members is not fused (use log_prob(x) of the result)");
     if (B == 0) return ZK_OK;
     const int64_t Bc = flow_chunk_rows(f, B, ws_bytes, 2);
     ZK_REQUIRE(Bc > 0, "flow_inverse: workspace too small (%zu < %zu)", ws_bytes, zk_flow_min_workspace_bytes(f));
@@ -1122,6 +1137,7 @@ zk_status zk_flow_log_prob_host(const zk_flow_desc* f, const float* xh, int64_t 
                                 int64_t ldc, int64_t B, float* lph, double* sum_host, void* ws,
                                 size_t ws_bytes, zk_stream stream) {
     ZK_TRY(flow_check(f));
+    ZK_TRY(inverted_members_run_forward(f));
     ZK_REQUIRE(xh && lph, "flow_log_prob_host: null argument");
     ZK_REQUIRE(B >= 0 && ldx >= f->features, "flow_log_prob_host: bad shape");
     ZK_REQUIRE(f->context == 0 || ch, "flow_log_prob_host: flow needs a context");
