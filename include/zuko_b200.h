@@ -261,7 +261,9 @@ zk_status zk_layer_destroy(zk_layer* layer);
  * bf16 hi / lo planes of the GEMM and fused kernels — with kernels on `stream`: no allocation, no
  * host synchronisation, no mask download.  The transposed weights of the backward pass and the
  * step-ordered stream of the sequential inverse are rebuilt by the next call that needs them.
- * weight / bias: host arrays of n_linear DEVICE pointers as in zk_mlp_desc (bias entries may be NULL).
+ * weight / bias: host arrays of n_linear DEVICE pointers as in zk_mlp_desc.  Unlike zk_mlp_desc, a NULL
+ * bias array or a NULL bias entry KEEPS that layer's current bias (it does not mean a zero bias).
+ * Every weight pointer is checked before any work is queued: a refusal (ZK_EINVAL) changes nothing.
  * Calls already queued on `stream` see the old weights, later ones the new. */
 zk_status zk_layer_update_weights(zk_layer* layer, const float* const* weight, const float* const* bias,
                                   zk_stream stream);
@@ -581,7 +583,8 @@ typedef struct zk_gmm zk_gmm;
 
 zk_status zk_gmm_create(const zk_gmm_desc* desc, zk_gmm** out);
 zk_status zk_gmm_destroy(zk_gmm* gmm);
-/* new conditioner weights / biases in place, as zk_layer_update_weights */
+/* new conditioner weights / biases in place, as zk_layer_update_weights (NULL bias entries keep the current
+ * bias; a refusal changes nothing) */
 zk_status zk_gmm_update_weights(zk_gmm* gmm, const float* const* weight, const float* const* bias, zk_stream stream);
 int64_t zk_gmm_params_per_row(int features, int components, int covariance, int tied);
 /* Launch plan of the mixture kernels (one thread per row, `threads` rows per CTA, per-row vectors in

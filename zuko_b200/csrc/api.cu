@@ -551,8 +551,9 @@ size_t zk_layer_workspace_bytes(const zk_layer* l, int64_t B) {
 namespace zkapi {
 
 zk_status mlp_update_weights(zk_mlp* m, const float* const* weight, const float* const* bias, cudaStream_t st) {
+    // every pointer is checked before the first launch: a refusal leaves all packed copies as they were
+    for (int i = 0; i < m->n_linear; ++i) ZK_REQUIRE(weight[i], "layer_update_weights: weight[%d] is null", i);
     for (int i = 0; i < m->n_linear; ++i) {
-        ZK_REQUIRE(weight[i], "layer_update_weights: weight[%d] is null", i);
         const int64_t n = (int64_t)m->dims[i + 1] * m->dims[i];
         ZK_TRY(launch_apply_mask(weight[i], m->mask[i], n, m->w[i], st));  // nn.py:218 `mask * W`, once per update
         if (bias && bias[i]) ZK_CUDA(cudaMemcpyAsync(m->b[i], bias[i], (size_t)m->dims[i + 1] * 4, cudaMemcpyDeviceToDevice, st));

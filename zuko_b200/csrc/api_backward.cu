@@ -52,6 +52,7 @@ zk_status mlp_ensure_backward(const zk_mlp* cm, cudaStream_t st) {
         ZK_TRY(launch_transpose(m->w[i], m->dims[i + 1], m->dims[i], t, st));
     }
     if (m->gemm_mode != ZK_GEMM_FP32 && m->tc != nullptr && m->act == 1 && m->plain) ZK_TRY(tc_pack_backward(m, st));
+    m->bwd_dirty = false;  // built from the current weights, so a refresh made before this backward is included
     ZK_CUDA(cudaStreamSynchronize(st));
     return ZK_OK;
 }
